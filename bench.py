@@ -1,15 +1,17 @@
 #!/usr/bin/env python
-"""bench.py -- subgraphs/sec of the MoCo pretraining step (BASELINE.json metric) on N x B200.
+"""bench.py -- subgraphs/sec of the MoCo pretraining step (BASELINE.json metric) on N x H100.
 
   python bench.py --gpus 1 --steps 50 --warmup 5                  (N>1: launched by torchrun)
   python bench.py --impl reference ...                            (CPU oracle arm, host cores)
+  python bench.py --steps 20 --dump-outputs DIR                   (also write the last timed step's outputs)
 
 Workload (config.workload): BASELINE.json configs[1] = "C2": MoCo K=16384 m=0.999, 5-layer GIN
 hid=64, rw_hops=256 restart=0.8, batch 256 (per GPU: weak scaling, configs[2] at N>1), synthetic
-power-law Chung-Lu graph 1M nodes / 20M edges (CSR ~168 MB > the 126 MB L2, sampled at random).
+power-law Chung-Lu graph 1M nodes / 20M edges (CSR ~168 MB > the 50 MB L2, sampled at random).
 One step = sample -> induce -> positional features -> GIN q/k -> InfoNCE -> backward -> clip/Adam
 -> EMA -> enqueue = 2*B ego-subgraphs.  `value` has inputs resident in HBM; `e2e` drives the same
 step with host-side seeds (pinned -> H2D) and a loss read-back (D2H) inside the timed region.
+Inputs (graph, seeds, initial weights, queue) are seeded: identical from run to run with the same arguments.
 """
 import argparse
 import contextlib
@@ -38,7 +40,7 @@ CONFIGS = {
 def parse():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=200)
+    ap.add_argument("--steps", type=int, default=200, help="timed steps (>= 1)")
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--config", default="c2", choices=sorted(CONFIGS))
@@ -49,7 +51,12 @@ def parse():
                          "views through the query encoder, in-batch negatives, no queue / momentum encoder)")
     ap.add_argument("--prefetch", type=int, default=4, choices=[1, 2, 3, 4, 5, 6, 8],
                     help="batches the sampler/eigensolver streams run ahead of the training stream")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    return args
 
 
 def workload_name(cfg, n_gpus):
@@ -338,6 +345,8 @@ def run_ours(args, cfg):
     ev[1].record()
     barrier()
     ms = ev[0].elapsed_time(ev[1])
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, eng, model, ema, contrast)
     per_step = [ev[0].elapsed_time(step_ev[0])] + [step_ev[i - 1].elapsed_time(step_ev[i]) for i in range(1, args.steps)]
     ps = sorted(per_step)
     med = ps[len(ps) // 2]
@@ -376,22 +385,14 @@ def run_ours(args, cfg):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak_gbs = float(peaks.get("hbm_gbs", 6650.0))
+    peak_gbs = float(peaks.get("hbm_gbs", 3350.0))
     achieved = alg_bytes / (samp_ms / 1e3) / 1e9
     roofline = {"kernel": "sampler: rwr_walk_unique + batch_offsets + induce_fill (per step, 3 launches)",
                 "bound": "hbm", "achieved": achieved, "peak": peak_gbs, "unit": "GB/s",
                 "frac": achieved / peak_gbs, "traffic": None,
-                "peak_source": "measured (MEASURED_PEAKS.json)" if peaks else "fallback 6650 GB/s",
+                "peak_source": "measured (MEASURED_PEAKS.json)" if peaks else "H100 SXM data sheet, 3350 GB/s",
                 "algorithmic_bytes_per_step": alg_bytes, "ms_per_launch_group": samp_ms,
                 "note": "latency-bound at %d ego-nets/step (tens of MB per launch group); see DESIGN.md" % (2 * B)}
-    try:
-        if args.config != "c2":
-            raise KeyError("the ncu capture is of the C2 workload")
-        tr = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-        roofline["traffic"] = tr["sampler_group_dram_bytes_per_step"]
-        roofline["traffic_source"] = tr.get("source", "profiles/traffic.json")
-    except Exception:
-        pass
     eig = eigensolver_report(eng.cur_buf, eig_ms)
     phases = {"sampler_ms": samp_ms, "eigensolver_ms": eig_ms, "step_ms": ms / args.steps,
               "note": "sampler + eigensolver of batch t+1 run on the data stream concurrently with the "
@@ -500,7 +501,7 @@ def eigensolver_report(buf, eig_ms):
     dense = 4.0 / 3.0 * n ** 3 + 128.0 * n ** 2 + 4096.0 * n + 768.0 * n + 7 * 256 * 5.0 * n
     flops = np.where(ch, deg_sum * (2 * (m + n) + 3 * n) * 48 + it * per_iter, np.where(it < 0, -it * 4.0 * n ** 3, dense))
     total = float(flops.sum())
-    peak = 148 * 128 * 2 * 1.965e9 / 1e12                   # fp32 FMA on the CUDA cores at 1965 MHz
+    peak = 132 * 128 * 2 * 1.98e9 / 1e12                    # fp32 FMA on the CUDA cores of an H100 SXM at 1980 MHz
     ach = total / (eig_ms / 1e3) / 1e12
     return {"bound": "fp32 CUDA-core FMA + shared-memory/barrier latency (neither HBM nor tensor; SURVEY 8d)",
             "k": 32, "block": 48, "egonets": int(len(n)), "mean_n": float(n.mean()), "max_n": int(n.max()),
@@ -509,6 +510,33 @@ def eigensolver_report(buf, eig_ms):
             "max_iterations": int(it.max()), "max_residual": float(res.max()),
             "est_flop_per_batch": total, "achieved": ach, "peak": peak, "unit": "TFLOP/s",
             "frac": ach / peak, "ms_per_batch": eig_ms, "egonets_per_sec": len(n) / (eig_ms / 1e3)}
+
+
+def dump_outputs(path, eng, model, ema, contrast):
+    """--dump-outputs: what the last timed step handed to its caller -- this step's loss / prob / grad norm, the
+    query and key embeddings, the Adam-updated weights, the momentum-updated key encoder, the queue after the
+    enqueue, and the positional features of the batch it trained on -- one float32 .npy per array.  An array
+    above 8 MB is replaced by a fixed, seeded sample of its rows, so the directory stays under 64 MB.
+    The inputs are identical from run to run; the float64 atomics of the BatchNorm statistics are not ordered, and
+    training amplifies that last-bit noise step after step, so a tight comparison of two builds uses a short run
+    (--warmup 0 --steps 1)."""
+    import numpy as np
+    import torch
+    torch.cuda.synchronize()
+    buf, B = eng.cur_buf, eng.B
+    arrays = {"stats": eng.stats, "feat_q": eng.feat_q, "feat_k": eng.feat_k,
+              "params": model.flat_params[:model.n_live], "params_ema": ema.flat_params[:model.n_live],
+              "queue": contrast.memory}
+    for v in (0, 1):
+        arrays["pos_view%d" % v] = buf.pos[v, :int(buf.node_off[v, B])]
+    cap = 8 << 20
+    os.makedirs(path, exist_ok=True)
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy()
+        if a.nbytes > cap:
+            keep = cap // (a.nbytes // a.shape[0])
+            a = a[np.sort(np.random.RandomState(0).choice(a.shape[0], keep, replace=False))]
+        np.save(os.path.join(path, name + ".npy"), a)
 
 
 _REAL_STDOUT = None

@@ -1,4 +1,4 @@
-"""gcc_b200: the THUDM/GCC pretraining hot path on B200 (sm_100a) -- see DESIGN.md."""
+"""gcc_b200: the THUDM/GCC pretraining hot path on H100 (sm_90a) -- see DESIGN.md."""
 import os as _os
 
 # The pretraining step keeps ~25 CUDA streams busy (training, key encoder, weight gradients, three

@@ -1,7 +1,7 @@
 """Loader for libgccb200.so -- the only compute path of this package.
 
-There is deliberately NO fallback: if the CUDA library is missing or no sm_100
-device is present, every compute entry point raises.  (The CPU oracle under
+There is deliberately NO fallback: if the CUDA library is missing or no sm_90
+(Hopper) device is present, every compute entry point raises.  (The CPU oracle under
 oracle/ is test infrastructure and is never imported from here.)
 """
 import ctypes
@@ -45,17 +45,17 @@ _arch = None
 
 
 def require_device():
-    """Fail loudly unless a Blackwell-class CUDA device is current."""
+    """Fail loudly unless a Hopper (compute capability 9.0) CUDA device is current."""
     global _arch
     if _arch is not None:
         return _arch
     import torch
     if not torch.cuda.is_available():
-        raise GccbError("gcc_b200 needs a CUDA device (sm_100a); none is visible and there is "
+        raise GccbError("gcc_b200 needs a CUDA device (sm_90a); none is visible and there is "
                         "no CPU fallback.")
     arch = get().gccb_arch()
-    if arch < 100:
-        raise GccbError("gcc_b200 kernels are built for sm_100a only; current device reports "
+    if arch != 90:                    # sm_90a code loads on compute capability 9.0 only
+        raise GccbError("gcc_b200 kernels are built for sm_90a only; current device reports "
                         "compute capability %s" % arch)
     _arch = arch
     return arch

@@ -1,10 +1,9 @@
-"""Build libgccb200.so (hand-written sm_100a CUDA + the C ABI) with nvcc, in-tree.
+"""Build libgccb200.so (hand-written sm_90a CUDA + the C ABI) with nvcc, in-tree.
 
     python -m gcc_b200.csrc.build          # or: __graft_entry__.build()
 
 nvcc cross-compiles without a GPU.  The library lands next to the package
-(gcc_b200/libgccb200.so): git-ignored, but it travels to the GPU box with the
-repo snapshot.
+(gcc_b200/libgccb200.so, git-ignored), objects under gcc_b200/build/.
 """
 import glob
 import os
@@ -17,7 +16,7 @@ ROOT = os.path.dirname(PKG)
 LIB = os.path.join(PKG, "libgccb200.so")
 OBJ_DIR = os.path.join(PKG, "build")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 

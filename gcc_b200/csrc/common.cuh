@@ -1,7 +1,10 @@
-// common.cuh -- shared device/host helpers for libgccb200 (sm_100a).
+// common.cuh -- shared device/host helpers for libgccb200 (sm_90a).
 #pragma once
 #include <mutex>
 #include <stdint.h>
+
+// Streaming multiprocessors of the target GPU (H100 SXM: 132): sizes persistent grids and split-K partitions.
+#define GCCB_NUM_SMS 132
 
 #ifdef GCCB_EMU
 // tests/emu/cuda_emu.h: CPU emulation used ONLY by the `-m "not gpu"` kernel-logic

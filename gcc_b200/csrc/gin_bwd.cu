@@ -17,7 +17,7 @@
 
 namespace gccb {
 
-#define GCCB_WG_CHUNKS 148    // row chunks of the weight-gradient split-K
+#define GCCB_WG_CHUNKS GCCB_NUM_SMS    // row chunks of the weight-gradient split-K
 
 struct BwdLayout {            // byte offsets in the backward workspace
   size_t dh, g1[2], dz2[2], da, red, dS, dpool, part, total;   // g1/dz2 alternate between layers
@@ -53,7 +53,7 @@ inline BwdLayout make_bwd_layout(const GinDims& d, int B, int node_cap) {
     b.tB = take((size_t)b.DW * b.cap_pad * 2);
     b.coef1 = take((size_t)(d.L - 1) * 2 * d.H * 4);
     const int tiles = (d.H / 128) * 1;                      // 128-row output tiles of a [H x <=256] weight gradient
-    b.splits = 148 / tiles;
+    b.splits = GCCB_NUM_SMS / tiles;
     if (b.splits > b.cap_pad / 64) b.splits = b.cap_pad / 64;
     if (b.splits < 1) b.splits = 1;
     b.splitk = take((size_t)b.splits * d.H * b.DW * 4);
@@ -657,7 +657,7 @@ static int run_backward(const BwdArgs& a) {
   float* G = a.grads;
   const int DW = a.bl.DW;
   const int tiles = (cap + GCCB_TILE_ROWS - 1) / GCCB_TILE_ROWS;
-  const int grid = tiles < 592 ? tiles : 592;
+  const int grid = tiles < 4 * GCCB_NUM_SMS ? tiles : 4 * GCCB_NUM_SMS;
   const uint32_t keep = (uint32_t)fmin((1.0 - (double)d.drop_p) * 4294967296.0, 4294967295.0);
   // The input-gradient chain (dh -> BN reductions -> GEMM2 -> GEMM1 -> next layer) is the critical
   // path; weight / BatchNorm / head gradients only consume its by-products, so they run on a side
@@ -786,7 +786,7 @@ static int run_backward(const BwdArgs& a) {
 #ifndef GCCB_EMU
 // ================================================================================================
 // Tensor-core backward (cfg.tensor_cores, hidden >= 128): the four GEMMs of a layer -- dx1 = dz2 W2,
-// da = dz1 W1, dW2 = dz2^T x1, dW1 = dz1^T a -- run on tcgen05 (csrc/tc_gemm.cu); the BatchNorm-backward
+// da = dz1 W1, dW2 = dz2^T x1, dW1 = dz1^T a -- run on wgmma (csrc/tc_gemm.cu); the BatchNorm-backward
 // chains between them are the same arithmetic as the SIMT kernels above, as elementwise passes that also
 // emit the bf16 operand of the next GEMM.  The biases of the two Linear layers feed train-mode BatchNorms:
 // their true gradient is exactly zero (the SIMT path computes rounding noise ~1e-9 there); this path adds
@@ -998,7 +998,7 @@ static int run_backward_tc(const BwdArgs& a) {
   float* G = a.grads;
   const int DW = a.bl.DW, capP = a.bl.cap_pad;
   const int tiles = (cap + GCCB_TILE_ROWS - 1) / GCCB_TILE_ROWS;
-  const int grid = tiles < 592 ? tiles : 592;
+  const int grid = tiles < 4 * GCCB_NUM_SMS ? tiles : 4 * GCCB_NUM_SMS;
   const uint32_t keep = (uint32_t)fmin((1.0 - (double)d.drop_p) * 4294967296.0, 4294967295.0);
   StreamKit* kit = stream_kit((cudaStream_t)a.stream, 1);
   cudaStream_t main_s = (cudaStream_t)a.stream;

@@ -12,7 +12,7 @@ namespace gccb {
 struct GinDims {
   int L, H, P, D, maxdeg, din;   // din = P + D + 1 (49)
   int norm;
-  int tc;                        // 1: Linear layers / their gradients on tcgen05 tensor cores (bf16 operands)
+  int tc;                        // 1: Linear layers / their gradients on wgmma tensor cores (bf16 operands)
   float bn_eps, bn_mom, norm_eps, drop_p;
 };
 
@@ -104,7 +104,7 @@ inline int dims_from_cfg(const gccb_gin_cfg_t* c, GinDims* d) {
 #ifdef GCCB_EMU
   d->tc = 0;                                              // the CPU emulator has no tensor cores
 #else
-  d->tc = (c->tensor_cores && c->hidden >= 128) ? 1 : 0;  // tcgen05 tiles are 128 x {128, 256}: hidden 32 / 64 stay SIMT fp32
+  d->tc = (c->tensor_cores && c->hidden >= 128) ? 1 : 0;  // tensor-core tiles are 128 x {128, 256}: hidden 32 / 64 stay SIMT fp32
 #endif
   if (d->L < 2 || d->L > GCCB_MAX_L || (d->H != 32 && d->H != 64 && d->H != 128 && d->H != 256) ||
       d->din > GCCB_DINP || d->P < 2 || d->P > 32 || d->D < 1 || d->maxdeg < 1) {

@@ -498,7 +498,7 @@ static int run_forward(const FwdArgs& a) {
   float* x0 = (float*)(a.acts + a.al.x0);
   double* stats = (double*)(a.acts + a.al.stats);
   const int tiles = (cap + GCCB_TILE_ROWS - 1) / GCCB_TILE_ROWS;
-  const int grid = tiles < 592 ? tiles : 592;            // 4 waves of 148 SMs at most
+  const int grid = tiles < 4 * GCCB_NUM_SMS ? tiles : 4 * GCCB_NUM_SMS;   // 4 waves at most
   const int use_running = a.bn_train ? 0 : 1, upd = a.bn_train ? 1 : 0;
   // BatchNorm statistics and the pooling accumulators are adjacent: one memset
   cudaMemsetAsync(stats, 0, a.al.pool_acc + (size_t)d.L * B * a.al.PW * sizeof(double) - a.al.stats,
@@ -563,8 +563,8 @@ static int run_forward(const FwdArgs& a) {
 #ifndef GCCB_EMU
 // ================================================================================================
 // Tensor-core path (cfg.tensor_cores, hidden >= 128; BASELINE config 4): the two Linear layers of every
-// GIN MLP (gin.py:113-116) run as tcgen05 GEMMs (csrc/tc_gemm.cu) with bf16 operands staged by TMA and
-// fp32 accumulation in TMEM; bias add and the BatchNorm column statistics are the GEMM epilogue.  The
+// GIN MLP (gin.py:113-116) run as wgmma GEMMs (csrc/tc_gemm.cu) with bf16 operands staged by TMA and
+// fp32 accumulation in registers; bias add and the BatchNorm column statistics are the GEMM epilogue.  The
 // gather / segmented reduce and the BatchNorm + ReLU between the GEMMs are bandwidth-bound passes that
 // also emit the bf16 operand of the next GEMM.  Activations stay fp32 in the stash (the backward's
 // elementwise chain is unchanged).
@@ -711,7 +711,7 @@ static int run_forward_tc(const FwdArgs& a) {
   __nv_bfloat16* a16 = (__nv_bfloat16*)(a.acts + a.al.a16);
   __nv_bfloat16* x16 = (__nv_bfloat16*)(a.acts + a.al.x16);
   const int tiles = (cap + GCCB_TILE_ROWS - 1) / GCCB_TILE_ROWS;
-  const int grid = tiles < 592 ? tiles : 592;
+  const int grid = tiles < 4 * GCCB_NUM_SMS ? tiles : 4 * GCCB_NUM_SMS;
   const int use_running = a.bn_train ? 0 : 1, upd = a.bn_train ? 1 : 0;
   cudaMemsetAsync(stats, 0, a.al.pool_acc + (size_t)d.L * B * a.al.PW * sizeof(double) - a.al.stats, st);
   GCCB_LAUNCH(gin_build_x0_kernel, grid, 256, 0, a.stream, d, node_off_v, B, pos_v, sub_deg, graph_id,

@@ -397,7 +397,7 @@ e2e_grads_kernel(const float* __restrict__ q, const float* __restrict__ k, const
 #ifndef GCCB_EMU
 // ---- tensor-core InfoNCE (d >= 128: BASELINE config 4, K = 65536, B = 1024, d = 256) ------------------------
 // logits = (q . queue^T) / T and dq = P . queue are the two big products of memory_moco.py:33-44 and its
-// backward; both run on tcgen05 (csrc/tc_gemm.cu) with bf16 operands: the queue is cast once per step into a
+// backward; both run on wgmma (csrc/tc_gemm.cu) with bf16 operands: the queue is cast once per step into a
 // [K][d] copy (B operand of the logits GEMM) and a transposed [d][K] copy (B operand of the dq GEMM, split-K
 // over the keys).  Between them one CTA per query row does the softmax in fp32 on the fp32 logits: loss,
 // probabilities (bf16 operand of the second GEMM) and the positive-pair terms.
@@ -414,7 +414,7 @@ static NceTcLayout nce_tc_layout(int B, int d, int K) {
   L.ppos = take((size_t)B * 4);
   L.dqn = take((size_t)B * d * 4);
   const int tiles = ((B + 127) / 128) * 1;
-  L.splits = 148 / tiles < 1 ? 1 : 148 / tiles;
+  L.splits = GCCB_NUM_SMS / tiles < 1 ? 1 : GCCB_NUM_SMS / tiles;
   if (L.splits > K / 64) L.splits = K / 64;
   L.splitk = take((size_t)L.splits * B * d * 4);
   L.total = off;

@@ -93,7 +93,7 @@ extern "C" int gccb_clip_adam_ema(float* p, float* g, float* m, float* v, float*
   }
   cudaMemsetAsync(workspace, 0, sizeof(double), (cudaStream_t)stream);
   int blocks = (int)((n_live + 255) / 256);
-  if (blocks > 592) blocks = 592;
+  if (blocks > 4 * GCCB_NUM_SMS) blocks = 4 * GCCB_NUM_SMS;
   GCCB_LAUNCH(gradnorm_kernel, blocks, 256, 0, stream, (const float*)g, n_live, grad_scale, workspace);
   int blocks2 = (int)((n_all + 255) / 256);
   if (blocks2 > 1184) blocks2 = 1184;

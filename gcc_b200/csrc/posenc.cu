@@ -89,19 +89,19 @@ namespace gccb {
 #define GCCB_CF_SMEM_PAD_A 0       // A/B builds: extra shared memory per n <= 96 CTA (lowers its CTAs per SM)
 #endif
 #ifndef GCCB_CAP_MID1
-#define GCCB_CAP_MID1 (148 * 3)     // persistent grid of the n <= 96 class (3 CTAs per SM)
+#define GCCB_CAP_MID1 (GCCB_NUM_SMS * 3)     // persistent grid of the n <= 96 class (3 CTAs per SM)
 #endif
 #ifndef GCCB_CAP_MID2
-#define GCCB_CAP_MID2 (148 * 2)     // persistent grid of the n <= 160 class (2 CTAs per SM)
+#define GCCB_CAP_MID2 (GCCB_NUM_SMS * 2)     // persistent grid of the n <= 160 class (2 CTAs per SM)
 #endif
 #ifndef GCCB_CAP_DN_A
-#define GCCB_CAP_DN_A (148 * 4)     // persistent grids of the dense classes
+#define GCCB_CAP_DN_A (GCCB_NUM_SMS * 4)     // persistent grids of the dense classes
 #endif
 #ifndef GCCB_CAP_DN_B
-#define GCCB_CAP_DN_B (148 * 2)
+#define GCCB_CAP_DN_B (GCCB_NUM_SMS * 2)
 #endif
 #ifndef GCCB_CAP_DN_C
-#define GCCB_CAP_DN_C 148
+#define GCCB_CAP_DN_C GCCB_NUM_SMS
 #endif
 #ifndef GCCB_BIG_NT
 #define GCCB_BIG_NT 512            // threads of the large-ego-net CTAs: 512 x 64 registers leave half of
@@ -2106,11 +2106,9 @@ extern "C" size_t gccb_posenc_workspace(int32_t batch, int32_t node_cap) {
          ((size_t)3 * 2 * batch + 4) * sizeof(int32_t);        // work lists + counts of the dense solver (tail)
 }
 
-// Largest ego-net handed to the dense tridiagonal solver.  Default: its first class, n <= 96 -- the only one that
-// beats the subspace iteration inside the running pipeline (C2 bench on one box, profiles/r02_dense_ab_c2.json:
-// 240.4k subgraphs/s without it, 265.4k with n <= 96, 256.8k with n <= 144, 244.6k with n <= 228: the larger
-// classes hold 108 / 224 KB of shared memory and 512 threads x 64 registers per CTA and crowd the training kernels
-// out of their SMs).  GCCB200_DENSE_MAX overrides (0 = ChFSI / Jacobi for every size, 228 = direct-method accuracy
+// Largest ego-net handed to the dense tridiagonal solver.  Default: its first class, n <= 96 -- the larger classes
+// hold 108 / 224 KB of shared memory and 512 threads x 64 registers per CTA and crowd the training kernels that run
+// beside them in the pipeline out of their SMs.  GCCB200_DENSE_MAX overrides (0 = ChFSI / Jacobi for every size, 228 = direct-method accuracy
 // for every ego-net up to 228 vertices); read on every call so that a test can compare the solvers in one process.
 static int posenc_dense_max() {
   const char* e = getenv("GCCB200_DENSE_MAX");
@@ -2215,9 +2213,8 @@ extern "C" int gccb_posenc(const gccb_batch_t* batch, int32_t pos_dim, int32_t n
     // dense classes: n <= 96 (256 threads, 48 KB: four CTAs per SM), n <= 144 (512 threads, 108 KB: two per SM),
     // n <= 228 (512 threads, 224 KB: one per SM); on the streams of the ChFSI classes they replace
     // GCCB200_DN_USM=1: class A keeps the factor rows of the inverse iteration in shared memory (74 KB per CTA, three
-    // per SM) instead of the L2 workspace (50 KB, four per SM).  Measured on the C2 bench (profiles/
-    // r02_dense_ab2_c2.json): 261.4k subgraphs/s against 265.2k -- the shorter inverse iteration does not pay for
-    // the larger footprint -- so it stays off.
+    // per SM) instead of the L2 workspace (50 KB, four per SM): a shorter inverse iteration for a larger footprint,
+    // off by default.
     const char* usm_e = getenv("GCCB200_DN_USM");
     const bool usm = usm_e && usm_e[0] == '1';
     auto kd_a = usm ? posenc_dense_kernel<GCCB_DN_A, 256, true> : posenc_dense_kernel<GCCB_DN_A, 256, false>;
@@ -2241,14 +2238,14 @@ extern "C" int gccb_posenc(const gccb_batch_t* batch, int32_t pos_dim, int32_t n
       GCCB_LAUNCH(kd_c, capped(env_cap("GCCB200_DN_CAP_C", GCCB_CAP_DN_C)), 512, sd_c, s_big, GCCB_DN_ARGS(2));
     if (dense_max > GCCB_DN_A)
       GCCB_LAUNCH(kd_b, capped(env_cap("GCCB200_DN_CAP_B", GCCB_CAP_DN_B)), 512, sd_b, s_mid2, GCCB_DN_ARGS(1));
-    GCCB_LAUNCH(kd_a, capped(env_cap("GCCB200_DN_CAP_A", usm ? 148 * 3 : GCCB_CAP_DN_A)), 256, sd_a, s_mid1, GCCB_DN_ARGS(0));
+    GCCB_LAUNCH(kd_a, capped(env_cap("GCCB200_DN_CAP_A", usm ? GCCB_NUM_SMS * 3 : GCCB_CAP_DN_A)), 256, sd_a, s_mid1, GCCB_DN_ARGS(0));
   }
-  GCCB_LAUNCH(kbig, capped(148), GCCB_BIG_NT, s_c, s_big, GCCB_PE_ARGS(3));
+  GCCB_LAUNCH(kbig, capped(GCCB_NUM_SMS), GCCB_BIG_NT, s_c, s_big, GCCB_PE_ARGS(3));
   // classes the dense solver covers completely have empty lists: not launched
   if (dense_max < GCCB_CF_NSM) GCCB_LAUNCH(kmid, capped(GCCB_CAP_MID2), 256, s_b, s_mid2, GCCB_PE_ARGS(2));
   if (dense_max < GCCB_CF_NSM_A) GCCB_LAUNCH(kmid, capped(GCCB_CAP_MID1), 256, s_a, s_mid1, GCCB_PE_ARGS(1));
   if (dense_max < GCCB_EIG_SMALL)
-    GCCB_LAUNCH(ksmall, capped(148), 256, 0, s_small, worklist, counts, B, batch->node_cap, batch->edge_cap,
+    GCCB_LAUNCH(ksmall, capped(GCCB_NUM_SMS), 256, 0, s_small, worklist, counts, B, batch->node_cap, batch->edge_cap,
                 batch->node_off, batch->indptr, batch->indices, batch->sub_deg, pos_dim, normalize, pos, eigvals,
                 batch->flags, dbg_iters, dbg_res);
 #ifndef GCCB_EMU

@@ -7,7 +7,7 @@
 //     g.subgraph, seed one-hot)                            gcc/datasets/data_util.py:218-239
 //   batcher() / dgl.batch                                  gcc/datasets/data_util.py:26-32
 //
-// Design (B200): one CTA per (sample, view).  Trace lengths depend only on the
+// Design (H100): one CTA per (sample, view).  Trace lengths depend only on the
 // counter-based RNG, so the stopping trace T* is found without touching memory;
 // then all traces are walked in parallel (dependent-load depth = longest single
 // trace, not the whole budget).  The visited list is bitonic-sorted / uniqued in

@@ -1,4 +1,4 @@
-// tc_gemm.cu -- the path's dense contraction on Blackwell tensor cores (tcgen05 + TMEM + TMA).
+// tc_gemm.cu -- the path's dense contraction on Hopper tensor cores (wgmma + TMA + mbarrier).
 //
 //   D[M x N] = alpha * A[M x K] . B[N x K]^T (+ bias[N])      A, B bf16 (K-major), fp32 accumulate
 //
@@ -10,14 +10,14 @@
 //   weight gradients dW = dZ^T . X     (operands transposed once, split-K over the rows)
 //   MoCo logits q . queue^T            (gcc/contrastive/memory_moco.py:33-44) and dq = P . queue
 // Design (one CTA per SM, persistent over 128-row output tiles):
-//   warp 0    TMA producer: cp.async.bulk.tensor 2-D boxes (128 x 64 of A, BN x 64 of B, 128-byte
+//   warp 8    TMA producer: cp.async.bulk.tensor 2-D boxes (128 x 64 of A, BN x 64 of B, 128-byte
 //             swizzle) into a 4-stage shared-memory ring, completion on mbarriers;
-//   warp 1    allocates TMEM and issues tcgen05.mma.cta_group::1.kind::f16 (M 128, N = BN, K 16) from
-//             one elected lane; tcgen05.commit releases the ring slot / publishes the accumulator;
-//   warps 2-5 epilogue: tcgen05.ld (32 lanes x 32 columns per warp), bias / scale, fp32 and/or bf16
-//             stores, column sums and sums of squares (float64 atomics, like the SIMT kernels).
-//   Two accumulator stages in TMEM (2 x BN <= 512 columns): the epilogue of tile t overlaps the
-//   MMAs of tile t+1.
+//   warps 0-7 two consumer warpgroups, rows 0-63 and 64-127 of the tile: wgmma.mma_async m64 x BN x 16
+//             with the fp32 accumulator in registers, one wgmma group in flight while the ring slot of
+//             the previous one is released; then the epilogue straight from the registers: bias / scale,
+//             fp32 and/or bf16 stores, column sums and sums of squares (float64 atomics, like the SIMT
+//             kernels).  The producer keeps filling the ring during the epilogue, so the MMAs of the
+//             next tile start on operands already in shared memory.
 // Shared-memory operand layout = the canonical K-major SWIZZLE_128B layout (8-row groups 1024 B apart),
 // which is exactly what a TMA box with CU_TENSOR_MAP_SWIZZLE_128B writes.
 #include "tc_gemm.cuh"
@@ -29,17 +29,12 @@
 namespace gccb {
 namespace tc {
 
-constexpr int BM = 128, BK = 64, STAGES = 4, UMMA_K = 16;
+constexpr int BM = 128, BK = 64, STAGES = 4, MMA_K = 16;
 constexpr int BIAS_SMEM = 512;                             // floats of bias staged in shared memory
-// Epilogue warps: a warp may only touch the TMEM lane group (warp % 4), so the 128 accumulator rows always need
-// 4 warps; wide tiles are split by COLUMNS over PARTS such sets (BN = 256: 16 warps of 64 columns each).  One
-// epilogue warp per scheduler issues an instruction every ~5 cycles (ncu: 18 % issue-slot use, the tile loop was
-// bound by this warp's dependent chain, not by TMA or the tensor pipe); four per scheduler hide each other.
-template <int BN> struct Epi {
-  static constexpr int PARTS = BN >= 256 ? 4 : BN >= 128 ? 2 : 1;
-  static constexpr int WARPS = 4 * PARTS, THREADS_EPI = 32 * WARPS, THREADS = 64 + THREADS_EPI;
-  static constexpr int COLS = BN / PARTS;                  // columns per warp (a multiple of 32)
-};
+// Two consumer warpgroups (rows 0-63 and 64-127 of the tile) and one TMA producer warp.  The accumulator lives in
+// registers (BN / 2 floats per consumer thread: 128 at BN = 256), so one CTA of 288 threads per SM (<= 224
+// registers per thread) holds a full 128 x 256 tile.
+constexpr int CONSUMERS = 256, THREADS = CONSUMERS + 32, CONSUMER_WARPS = CONSUMERS / 32;
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -76,32 +71,101 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, i
       "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// D[tmem] (+)= A[smem desc] . B[smem desc]^T
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(da), "l"(db), "r"(idesc), "r"(acc)
-      : "memory");
-}
-// K-major SWIZZLE_128B operand descriptor (cute::UMMA::SmemDescriptor): start address >> 4 in bits
-// [0,14), leading byte offset (unused for swizzled K-major) = 1 in [16,30), stride byte offset
-// (8-row group pitch, 1024 B) >> 4 in [32,46), version 1 in [46,48), layout type 2 = SWIZZLE_128B in [61,64).
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr) {
+// K-major SWIZZLE_128B wgmma matrix descriptor: start address >> 4 in bits [0,14), leading byte offset (unused for
+// swizzled K-major) = 1 in [16,30), stride byte offset (8-row group pitch, 1024 B) >> 4 in [32,46), base offset 0
+// (every tile is 1024-byte aligned), layout type 1 = SWIZZLE_128B in [62,64).
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t saddr) {
   return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) |
-         ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
+         ((uint64_t)1 << 62);
 }
-// cute::UMMA::InstrDescriptor: c_format F32 (1 << 4), a/b_format BF16 (1 << 7, 1 << 10), K-major both
-// (bits 15, 16 = 0), n_dim = N >> 3 at bit 17, m_dim = M >> 4 at bit 24.
-__host__ __device__ constexpr uint32_t umma_idesc(int m, int n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across an asynchronous wgmma
+template <int R>
+__device__ __forceinline__ void fence_acc(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// d[64 x BN] (+)= A[64 x 16 at da] . B[BN x 16 at db]^T, both operands K-major in shared memory.  The fragment of
+// thread t of the warpgroup: d[4 j + {0, 1, 2, 3}] = (row r, col 8 j + c), (r, c + 1), (r + 8, c), (r + 8, c + 1)
+// with r = 16 (warp % 4) + lane / 4, c = 2 (lane % 4).
+template <int BN>
+__device__ void wgmma_bf16(float* d, uint64_t da, uint64_t db, int acc);
+template <> __device__ __forceinline__ void wgmma_bf16<32>(float* d, uint64_t da, uint64_t db, int acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+      "}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma_bf16<64>(float* d, uint64_t da, uint64_t db, int acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+      "}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma_bf16<128>(float* d, uint64_t da, uint64_t db, int acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+      "}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma_bf16<256>(float* d, uint64_t da, uint64_t db, int acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+      "}, %128, %129, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(da), "l"(db), "r"(acc));
 }
 
 struct GemmArgs {
@@ -124,27 +188,60 @@ struct Smem {
   static constexpr int STAGE_BYTES = BRES ? A_BYTES : A_BYTES + B_BYTES;
   static constexpr int BRES_KB = 4;                        // k-blocks of the resident operand (K <= 256)
   static constexpr size_t BRES_BYTES = BRES ? (size_t)BRES_KB * B_BYTES : 0;
-  static constexpr int STAGE_F = 128 * 33;                 // epilogue transpose buffer (floats)
-  static constexpr size_t TOTAL = 1024 + BRES_BYTES + (size_t)STAGES * STAGE_BYTES + STAGE_F * 4 + 2 * 256 * 4 + 256;
+  static constexpr int COLACC_F = CONSUMER_WARPS * 2 * BN; // per-warp column sums / sums of squares
+  static constexpr size_t TOTAL =
+      1024 + BRES_BYTES + (size_t)STAGES * STAGE_BYTES + (size_t)(COLACC_F + BIAS_SMEM) * 4 + 256;
 };
 
+// Column sums over the 64 rows of a warpgroup's fragment without shared-memory traffic: x holds, for G 8-column
+// groups, (sum c, sum c + 1, sum of squares c, c + 1) of the thread's two rows.  The lanes sharing lane % 4 own the
+// same columns; a transpose-reduce over lane bits 4, 3, 2 (each exchange halves what a lane keeps) leaves group
+// lane >> (5 - log2 G) on the lane, fully summed over the warp's 16 rows; it is added to the warp's own row of accw.
+template <int N, int OFF>
+__device__ __forceinline__ void colsum_level(float* x, int lane) {
+  if constexpr (OFF >= 4) {
+    if constexpr (N > 4) {
+      const bool upper = (lane & OFF) != 0;
+#pragma unroll
+      for (int i = 0; i < N / 2; ++i) {
+        const float send = upper ? x[i] : x[i + N / 2], keep = upper ? x[i + N / 2] : x[i];
+        x[i] = keep + __shfl_xor_sync(0xffffffffu, send, OFF);
+      }
+      colsum_level<N / 2, OFF / 2>(x, lane);
+    } else {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) x[i] += __shfl_xor_sync(0xffffffffu, x[i], OFF);
+      colsum_level<4, OFF / 2>(x, lane);
+    }
+  }
+}
+template <int G>
+__device__ __forceinline__ void colstats_chunk(float (&x)[4 * G], int lane, float* accw, int BN, int col0) {
+  constexpr int LOG_G = G >= 8 ? 3 : G >= 4 ? 2 : G >= 2 ? 1 : 0;
+  colsum_level<4 * G, 16>(x, lane);
+  if (((lane >> 2) & ((1 << (3 - LOG_G)) - 1)) == 0) {
+    const int c = col0 + 8 * (lane >> (5 - LOG_G)) + 2 * (lane & 3);
+    accw[c] += x[0];
+    accw[c + 1] += x[1];
+    accw[BN + c] += x[2];
+    accw[BN + c + 1] += x[3];
+  }
+}
+
 template <int BN, bool BRES>
-__global__ void __launch_bounds__(Epi<BN>::THREADS, 1)
+__global__ void __launch_bounds__(THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, GemmArgs g) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   using S = Smem<BN, BRES>;
   unsigned char* base = (unsigned char*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   unsigned char* bres = base;                                        // [BRES_KB][B] (BRES only)
   unsigned char* tiles = base + S::BRES_BYTES;                       // [STAGES][A | B]  (BRES: [STAGES][A])
-  float* stage_t = (float*)(tiles + (size_t)STAGES * S::STAGE_BYTES);   // [128][33]
-  float* colpart = stage_t + S::STAGE_F;                              // [512]: bias staging
-  uint64_t* bars = (uint64_t*)(colpart + 2 * 256);
+  float* colacc = (float*)(tiles + (size_t)STAGES * S::STAGE_BYTES); // [CONSUMER_WARPS][2][BN]
+  float* bias_s = colacc + S::COLACC_F;                              // [BIAS_SMEM]
+  uint64_t* bars = (uint64_t*)(bias_s + BIAS_SMEM);
   uint64_t* full = bars;                 // [STAGES]   TMA -> MMA
   uint64_t* empty = bars + STAGES;       // [STAGES]   MMA -> TMA
-  uint64_t* tfull = bars + 2 * STAGES;   // [2]        MMA -> epilogue
-  uint64_t* tempty = bars + 2 * STAGES + 2;   // [2]   epilogue -> MMA
-  uint64_t* bfull = bars + 2 * STAGES + 4;    // [1]   resident B operand landed
-  uint32_t* tmem_slot = (uint32_t*)(bars + 2 * STAGES + 5);
+  uint64_t* bfull = bars + 2 * STAGES;   // [1]        resident B operand landed
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int M = g.m_dev ? min(max(*g.m_dev, 0), g.M_cap) : g.M_cap;
@@ -155,229 +252,136 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   const int kb0 = split * kb_per, kb1 = min(kb_total, kb0 + kb_per);
   const int nkb = max(kb1 - kb0, 0);
   const int num_tiles = m_tiles * n_tiles;
-  constexpr uint32_t TMEM_COLS = 2 * BN <= 32 ? 32 : 2 * BN <= 64 ? 64 : 2 * BN <= 128 ? 128 : 2 * BN <= 256 ? 256 : 512;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&tfull[i], 1); mbar_init(&tempty[i], Epi<BN>::WARPS); }
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], CONSUMER_WARPS); }
     mbar_init(bfull, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {                       // TMEM allocation: one full warp; the same warp frees it
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "n"(TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
   // bias (zeros when absent) in shared memory when it fits: the epilogue then needs no global loads
-  float* bias_s = colpart;                                            // [BIAS_SMEM]
   const bool bias_in_smem = g.N <= BIAS_SMEM;
   if (bias_in_smem)
     for (int i = threadIdx.x; i < g.N; i += blockDim.x) bias_s[i] = g.bias ? g.bias[i] : 0.f;
-  tc_fence_before();
+  if (g.colstats)
+    for (int i = threadIdx.x; i < S::COLACC_F; i += blockDim.x) colacc[i] = 0.f;
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if (nkb == 0) return;
 
-  if (nkb > 0) {
-    if (warp == 0) {
-      // ===== TMA producer ============================================================================
-      if (lane == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
-        int stage = 0;
-        uint32_t phase = 0;
-        if (BRES && blockIdx.x < num_tiles) {              // the whole B operand, once
-          mbar_expect_tx(bfull, (uint32_t)(nkb * S::B_BYTES));
-          for (int kb = 0; kb < nkb; ++kb) tma_load_2d(bres + (size_t)kb * S::B_BYTES, &map_b, kb * BK, 0, bfull);
-        }
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-          const int mt = tile / n_tiles, nt = tile - mt * n_tiles;
-          for (int kb = kb0; kb < kb1; ++kb) {
-            mbar_wait(&empty[stage], phase ^ 1);
-            unsigned char* sa = tiles + (size_t)stage * S::STAGE_BYTES;
-            mbar_expect_tx(&full[stage], S::STAGE_BYTES);
-            tma_load_2d(sa, &map_a, kb * BK, mt * BM, &full[stage]);
-            if (!BRES) tma_load_2d(sa + S::A_BYTES, &map_b, kb * BK, nt * BN, &full[stage]);
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-          }
-        }
-      }
-    } else if (warp == 1) {
-      // ===== MMA issuer (one elected lane) ===========================================================
-      if (lane == 0) {
-        constexpr uint32_t idesc = umma_idesc(BM, BN);
-        int stage = 0;
-        uint32_t phase = 0;
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        if (BRES && blockIdx.x < num_tiles) mbar_wait(bfull, 0);
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-          mbar_wait(&tempty[acc], acc_phase ^ 1);          // epilogue has drained this accumulator
-          tc_fence_after();
-          const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BN);
-          for (int kb = 0; kb < nkb; ++kb) {
-            mbar_wait(&full[stage], phase);
-            tc_fence_after();
-            const uint32_t sa = smem_u32(tiles + (size_t)stage * S::STAGE_BYTES);
-            const uint32_t sb = BRES ? smem_u32(bres + (size_t)kb * S::B_BYTES) : sa + S::A_BYTES;
-#pragma unroll
-            for (int k = 0; k < BK / UMMA_K; ++k) {
-              // advancing 16 elements (32 B) along K inside the 128-byte swizzle atom = +32 B on the start address
-              umma_bf16(d_tmem, umma_desc(sa + k * UMMA_K * 2), umma_desc(sb + k * UMMA_K * 2), idesc,
-                        (uint32_t)((kb | k) != 0));
-            }
-            umma_commit(&empty[stage]);                    // ring slot free once these MMAs have read it
-            if (kb == nkb - 1) umma_commit(&tfull[acc]);   // accumulator complete
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-          }
-          if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-        }
-      }
-    } else {
-      // ===== epilogue warps 2..: TMEM lanes 32 * (warp % 4) .. +31, columns [part * COLS, (part + 1) * COLS) ====
-      const int ew = warp & 3;                              // TMEM lane group this warp may access
-      const int part = (warp - 2) >> 2;
-      constexpr int COLS = Epi<BN>::COLS;
-      const int et = threadIdx.x - 64;                      // 0 .. THREADS_EPI - 1
-      const int row_in_tile = ew * 32 + lane;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      float* outf = g.out_f32 ? g.out_f32 + (size_t)split * g.M_cap * g.ldo : nullptr;
-      const bool wide_f32 = outf && ((((uintptr_t)outf) | ((size_t)g.ldo * 4)) & 31) == 0;
-      const bool wide_bf16 = g.out_bf16 && ((((uintptr_t)g.out_bf16) | ((size_t)g.ldo * 2)) & 31) == 0;
-      if (g.colstats) {                                     // per-warp column accumulators (n_tiles == 1 with statistics)
-        for (int i = lane; i < COLS; i += 32) {               // own columns only: the warps of a lane group share a row
-          stage_t[ew * (2 * BN) + part * COLS + i] = 0.f;
-          stage_t[ew * (2 * BN) + BN + part * COLS + i] = 0.f;
-        }
-        __syncwarp();
+  if (warp == CONSUMER_WARPS) {
+    // ===== TMA producer =============================================================================
+    if (lane == 0) {
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
+      int stage = 0;
+      uint32_t phase = 0;
+      if (BRES && blockIdx.x < num_tiles) {              // the whole B operand, once
+        mbar_expect_tx(bfull, (uint32_t)(nkb * S::B_BYTES));
+        for (int kb = 0; kb < nkb; ++kb) tma_load_2d(bres + (size_t)kb * S::B_BYTES, &map_b, kb * BK, 0, bfull);
       }
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int mt = tile / n_tiles, nt = tile - mt * n_tiles;
-        const int row = mt * BM + row_in_tile;
-        const bool row_ok = row < M;
-        const bool full_tile = (mt + 1) * BM <= M;
-        mbar_wait(&tfull[acc], acc_phase);
-        tc_fence_after();
-#pragma unroll 1
-        for (int c0 = part * COLS; c0 < (part + 1) * COLS; c0 += 32) {
-          uint32_t r[32];
-          const uint32_t taddr = tmem_base + ((uint32_t)(ew * 32) << 16) + (uint32_t)(acc * BN + c0);
-          asm volatile(
-              "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-              "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-              "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-              : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-                "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]),
-                "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]),
-                "=r"(r[30]), "=r"(r[31])
-              : "r"(taddr));
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-          const int col0 = nt * BN + c0;
-          float v[32];
-          if (bias_in_smem) {                               // bias (or zeros) staged in shared memory: 8 x LDS.128
-            const float4* b4 = reinterpret_cast<const float4*>(bias_s + col0);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float4 b = b4[j];
-              v[4 * j] = fmaf(__uint_as_float(r[4 * j]), g.alpha, b.x);
-              v[4 * j + 1] = fmaf(__uint_as_float(r[4 * j + 1]), g.alpha, b.y);
-              v[4 * j + 2] = fmaf(__uint_as_float(r[4 * j + 2]), g.alpha, b.z);
-              v[4 * j + 3] = fmaf(__uint_as_float(r[4 * j + 3]), g.alpha, b.w);
-            }
-          } else {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = fmaf(__uint_as_float(r[j]), g.alpha, g.bias ? g.bias[col0 + j] : 0.f);
-          }
-          if (!full_tile) {                                 // only the last row tile has rows to mask
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = row_ok ? v[j] : 0.f;
-          }
-          if (row_ok) {
-            // a TMEM lane holds one ROW: each lane stores its 32 columns itself.  256-bit stores (sm_100) when the
-            // row pitch allows: every store fills whole 32-byte sectors, half the store instructions
-            if (outf) {
-              float* dst = outf + (size_t)row * g.ldo + col0;
-              if (wide_f32) {
-#pragma unroll
-                for (int j = 0; j < 4; ++j)
-                  asm volatile("st.global.v8.f32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(dst + 8 * j),
-                               "f"(v[8 * j]), "f"(v[8 * j + 1]), "f"(v[8 * j + 2]), "f"(v[8 * j + 3]), "f"(v[8 * j + 4]),
-                               "f"(v[8 * j + 5]), "f"(v[8 * j + 6]), "f"(v[8 * j + 7])
-                               : "memory");
-              } else {
-                float4* d4 = reinterpret_cast<float4*>(dst);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) d4[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-              }
-            }
-            if (g.out_bf16) {
-              uint32_t pk[16];
-#pragma unroll
-              for (int j = 0; j < 16; ++j) {
-                __nv_bfloat162 p2 = __floats2bfloat162_rn(v[2 * j], v[2 * j + 1]);
-                pk[j] = *reinterpret_cast<uint32_t*>(&p2);
-              }
-              __nv_bfloat16* dst = g.out_bf16 + (size_t)row * g.ldo + col0;
-              if (wide_bf16) {
-#pragma unroll
-                for (int j = 0; j < 2; ++j)
-                  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(dst + 16 * j),
-                               "r"(pk[8 * j]), "r"(pk[8 * j + 1]), "r"(pk[8 * j + 2]), "r"(pk[8 * j + 3]), "r"(pk[8 * j + 4]),
-                               "r"(pk[8 * j + 5]), "r"(pk[8 * j + 6]), "r"(pk[8 * j + 7])
-                               : "memory");
-              } else {
-                uint4* d4 = reinterpret_cast<uint4*>(dst);
-#pragma unroll
-                for (int j = 0; j < 4; ++j) d4[j] = make_uint4(pk[4 * j], pk[4 * j + 1], pk[4 * j + 2], pk[4 * j + 3]);
-              }
-            }
-          }
-          if (g.colstats) {
-            // column sums over the warp's 32 rows without shared memory or barriers: a shuffle transpose-reduce
-            // (16 + 8 + 4 + 2 + 1 exchanges per quantity) leaves column `lane` of the chunk on lane `lane`; the
-            // warp then adds it to its private accumulator row (flushed once per CTA, below)
-            float q[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) q[j] = v[j] * v[j];
-#pragma unroll
-            for (int off = 16; off >= 1; off >>= 1) {
-              const bool upper = (lane & off) != 0;
-#pragma unroll
-              for (int i = 0; i < off; ++i) {
-                const float sv = upper ? v[i] : v[i + off], kv = upper ? v[i + off] : v[i];
-                v[i] = kv + __shfl_xor_sync(0xffffffffu, sv, off);
-                const float sq = upper ? q[i] : q[i + off], kq = upper ? q[i + off] : q[i];
-                q[i] = kq + __shfl_xor_sync(0xffffffffu, sq, off);
-              }
-            }
-            float* accw = stage_t + ew * (2 * BN);          // [4 warps][2][BN] floats (BN <= 256: 8 KB of the 16.5 KB)
-            accw[c0 + lane] += v[0];
-            accw[BN + c0 + lane] += q[0];
-          }
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tempty[acc]);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-      if (g.colstats) {                                     // one float64 atomic per column and CTA
-        asm volatile("bar.sync 1, %0;" ::"n"(Epi<BN>::THREADS_EPI) : "memory");
-        for (int i = et; i < 2 * BN; i += Epi<BN>::THREADS_EPI) {
-          const float t = stage_t[i] + stage_t[2 * BN + i] + stage_t[4 * BN + i] + stage_t[6 * BN + i];
-          const int which = i / BN, c = i - which * BN;
-          if (blockIdx.x < num_tiles) atomicAdd(&g.colstats[(size_t)which * g.N + c], (double)t);
+        for (int kb = kb0; kb < kb1; ++kb) {
+          mbar_wait(&empty[stage], phase ^ 1);
+          unsigned char* sa = tiles + (size_t)stage * S::STAGE_BYTES;
+          mbar_expect_tx(&full[stage], S::STAGE_BYTES);
+          tma_load_2d(sa, &map_a, kb * BK, mt * BM, &full[stage]);
+          if (!BRES) tma_load_2d(sa + S::A_BYTES, &map_b, kb * BK, nt * BN, &full[stage]);
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
     }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS) : "memory");
+
+  // ===== consumer warpgroups: MMA, then the epilogue from registers ==================================
+  const int wg = warp >> 2;                                  // rows 64 wg .. 64 wg + 63 of the tile
+  const int r_lo = 64 * wg + 16 * (warp & 3) + (lane >> 2);  // this thread's rows: r_lo, r_lo + 8
+  const int cq = 2 * (lane & 3);                             // and columns 8 j + cq, 8 j + cq + 1
+  float* outf = g.out_f32 ? g.out_f32 + (size_t)split * g.M_cap * g.ldo : nullptr;
+  float* accw = colacc + warp * (2 * BN);
+  float acc[BN / 2];
+  int stage = 0;
+  uint32_t phase = 0;
+  if (BRES && blockIdx.x < num_tiles) mbar_wait(bfull, 0);
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    const int mt = tile / n_tiles, nt = tile - mt * n_tiles;
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int prev = 0;
+    for (int kb = 0; kb < nkb; ++kb) {
+      mbar_wait(&full[stage], phase);
+      const uint32_t st = smem_u32(tiles + (size_t)stage * S::STAGE_BYTES);
+      const uint32_t sa = st + wg * (64 * BK * 2);
+      const uint32_t sb = BRES ? smem_u32(bres + (size_t)kb * S::B_BYTES) : st + S::A_BYTES;
+      fence_acc(acc);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / MMA_K; ++k)
+        // advancing 16 elements (32 B) along K inside the 128-byte swizzle atom = +32 B on the start address
+        wgmma_bf16<BN>(acc, wgmma_desc(sa + k * MMA_K * 2), wgmma_desc(sb + k * MMA_K * 2), (kb | k) != 0);
+      wgmma_commit();
+      fence_acc(acc);
+      if (kb > 0) {                                          // one group in flight: the previous slot is free
+        wgmma_wait<1>();
+        fence_acc(acc);
+        if (lane == 0) mbar_arrive(&empty[prev]);
+      }
+      prev = stage;
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    fence_acc(acc);
+    if (lane == 0) mbar_arrive(&empty[prev]);
+
+    const int row0 = mt * BM + r_lo, row1 = row0 + 8;
+    const bool ok0 = row0 < M, ok1 = row1 < M;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int c = nt * BN + 8 * j + cq;
+      float2 b = make_float2(0.f, 0.f);
+      if (bias_in_smem) b = *reinterpret_cast<const float2*>(bias_s + c);
+      else if (g.bias) b = make_float2(g.bias[c], g.bias[c + 1]);
+      float* v = acc + 4 * j;
+      v[0] = ok0 ? fmaf(v[0], g.alpha, b.x) : 0.f;
+      v[1] = ok0 ? fmaf(v[1], g.alpha, b.y) : 0.f;
+      v[2] = ok1 ? fmaf(v[2], g.alpha, b.x) : 0.f;
+      v[3] = ok1 ? fmaf(v[3], g.alpha, b.y) : 0.f;
+      // 4 lanes store one 32-byte sector of a row: every store instruction fills whole sectors
+      if (outf) {
+        if (ok0) *reinterpret_cast<float2*>(outf + (size_t)row0 * g.ldo + c) = make_float2(v[0], v[1]);
+        if (ok1) *reinterpret_cast<float2*>(outf + (size_t)row1 * g.ldo + c) = make_float2(v[2], v[3]);
+      }
+      if (g.out_bf16) {
+        if (ok0) *reinterpret_cast<__nv_bfloat162*>(g.out_bf16 + (size_t)row0 * g.ldo + c) = __floats2bfloat162_rn(v[0], v[1]);
+        if (ok1) *reinterpret_cast<__nv_bfloat162*>(g.out_bf16 + (size_t)row1 * g.ldo + c) = __floats2bfloat162_rn(v[2], v[3]);
+      }
+    }
+    if (g.colstats) {                                        // n_tiles == 1 with statistics
+      constexpr int G = BN / 8 < 8 ? BN / 8 : 8;
+#pragma unroll
+      for (int ch = 0; ch < BN / (8 * G); ++ch) {
+        float x[4 * G];
+#pragma unroll
+        for (int i = 0; i < G; ++i) {
+          const float* v = acc + 4 * (ch * G + i);
+          x[4 * i] = v[0] + v[2];
+          x[4 * i + 1] = v[1] + v[3];
+          x[4 * i + 2] = v[0] * v[0] + v[2] * v[2];
+          x[4 * i + 3] = v[1] * v[1] + v[3] * v[3];
+        }
+        colstats_chunk<G>(x, lane, accw, BN, ch * 8 * G);
+      }
+    }
+  }
+  if (g.colstats) {                                          // one float64 atomic per column and CTA
+    asm volatile("bar.sync 1, %0;" ::"n"(CONSUMERS) : "memory");
+    for (int i = threadIdx.x; i < 2 * BN; i += CONSUMERS) {
+      float t = 0.f;
+#pragma unroll
+      for (int w = 0; w < CONSUMER_WARPS; ++w) t += colacc[w * 2 * BN + i];
+      const int which = i / BN, c = i - which * BN;
+      if (blockIdx.x < num_tiles) atomicAdd(&g.colstats[(size_t)which * g.N + c], (double)t);
+    }
   }
 }
 
@@ -443,7 +447,7 @@ int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = GCCB_NUM_SMS;
   }
   return n;
 }
@@ -459,7 +463,7 @@ static int launch(const CUtensorMap& ma, const CUtensorMap& mb, const GemmArgs& 
   if (gx > tiles) gx = tiles;
   dim3 grid(gx, g.splits);
   ++gccb::g_launch_count;
-  k<<<grid, Epi<BN>::THREADS, smem, stream>>>(ma, mb, g);
+  k<<<grid, THREADS, smem, stream>>>(ma, mb, g);
   return GCCB_OK;
 }
 
@@ -642,7 +646,7 @@ extern "C" int gccb_cast_bf16(const float* src, int32_t rows, int32_t cols, int3
   return tc::cast_bf16(src, rows, cols, lds, dst, rows_pad, cols_pad, transpose, rows_dev, (cudaStream_t)stream);
 }
 
-#else   // GCCB_EMU: the CPU emulator cannot run tcgen05 / TMA; the entry points report it
+#else   // GCCB_EMU: the CPU emulator cannot run wgmma / TMA; the entry points report it
 extern "C" int gccb_tc_gemm_bf16(const void*, const void*, int32_t, int32_t, int32_t, const int32_t*, const float*,
                                  float, float*, void*, int32_t, double*, int32_t, float*, gccb_stream_t) {
   gccb::set_last_error("tc_gemm: tensor-core path is not available under the CPU emulator");

@@ -1,4 +1,4 @@
-// tc_gemm.cuh -- internal interface of the tcgen05 contraction (csrc/tc_gemm.cu) for the GIN / MoCo paths.
+// tc_gemm.cuh -- internal interface of the wgmma contraction (csrc/tc_gemm.cu) for the GIN / MoCo paths.
 #pragma once
 #include "common.cuh"
 #ifndef GCCB_EMU

@@ -1,4 +1,4 @@
-"""Device-resident ego-net dataset: the B200 replacement of the reference's CPU DataLoader.
+"""Device-resident ego-net dataset: the GPU replacement of the reference's CPU DataLoader.
 
 Mirrors the surface of gcc/datasets/graph_dataset.py that train.py touches
 (LoadBalanceGraphDataset ctor kwargs, .total, .jobs, .dgl_graphs_file, iteration

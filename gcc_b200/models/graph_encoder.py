@@ -1,6 +1,6 @@
 """GraphEncoder with the reference's constructor, forward signature and state_dict keys
 (gcc/models/graph_encoder.py:19-200, gin branch; SURVEY.md section 8b), executing as
-hand-written sm_100a kernels through libgccb200 (csrc/gin_fwd.cu, csrc/gin_bwd.cu).
+hand-written sm_90a kernels through libgccb200 (csrc/gin_fwd.cu, csrc/gin_bwd.cu).
 
 All live parameters are views into ONE flat fp32 buffer (models/layout.py) followed by the
 unused-but-present tensors of the reference module (set2set.*, lin_readout.*), so that

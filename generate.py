@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""generate.py -- the reference's inference export (generate.py:33-134) on the B200 kernels.
+"""generate.py -- the reference's inference export (generate.py:33-134) on the H100 kernels.
 
 Loads a pretraining checkpoint (`--load-path`, written by this repo's train.py or by the reference:
 same `model` state_dict keys), walks two ego-nets from EVERY node of the target graph in order
@@ -58,7 +58,7 @@ def main(args_test):
     if not os.path.isfile(path):
         raise SystemExit("=> no checkpoint found at '{}'".format(path))
     if not torch.cuda.is_available():
-        raise SystemExit("generate.py needs a CUDA device (sm_100a); there is no CPU path")
+        raise SystemExit("generate.py needs a CUDA device (sm_90a); there is no CPU path")
     print("=> loading checkpoint '{}'".format(path))
     ckpt = torch.load(path, map_location="cpu", weights_only=False)
     print("=> loaded successfully '{}' (epoch {})".format(path, ckpt["epoch"]))

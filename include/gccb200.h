@@ -1,5 +1,5 @@
 /*
- * gccb200.h -- C ABI of libgccb200.so: the Blackwell (sm_100a) implementation of the
+ * gccb200.h -- C ABI of libgccb200.so: the Hopper (sm_90a) implementation of the
  * THUDM/GCC pretraining hot path (SURVEY.md section 8).
  *
  * The reference has no FFI of its own (it is Python calling DGL / PyTorch), so
@@ -12,7 +12,7 @@
  *     non-convergence) are reported through a device-side flag word
  *     (gccb_batch_t.flags, GCCB_FLAG_*), so calls stay CUDA-graph capturable;
  *   - stateless, thread-safe per stream.
- * There is no CPU fallback: on a machine without an sm_100 device every compute
+ * There is no CPU fallback: on a machine without an sm_90 device every compute
  * entry point returns GCCB_ERR_CUDA / GCCB_ERR_ARCH.
  */
 #ifndef GCCB200_H_
@@ -142,7 +142,7 @@ typedef struct {
   float norm_eps;      /* 1e-5 */
   float dropout_p;     /* 0.5 (gin.py:202)                                          */
   int32_t tensor_cores; /* 1: the Linear layers of the MLP (gin.py:107-116) and their input / weight
-                           gradients run on tcgen05 tensor cores with bf16 operands and fp32
+                           gradients run on wgmma tensor cores with bf16 operands and fp32
                            accumulation (hidden >= 128 only; BASELINE config 4); 0: fp32 SIMT  */
   int32_t _pad;
 } gccb_gin_cfg_t;
@@ -234,7 +234,7 @@ int gccb_clip_adam_ema(float* p, float* g, float* m, float* v, float* p_ema, int
 int gccb_sum_ranks(const float* gathered, int32_t world, int64_t stride, int64_t n, float* out,
                    int64_t flag_index, int32_t* any_flag_out, gccb_stream_t stream);
 
-/* ---- tensor-core contraction (tcgen05 + TMEM + TMA; csrc/tc_gemm.cu) ------------------------------
+/* ---- tensor-core contraction (wgmma + TMA; csrc/tc_gemm.cu) ---------------------------------------
  * The dense products of the path at hidden >= 128 (BASELINE config 4): the GIN MLP's Linear layers
  * (gcc/models/gin.py:107-116) with the BatchNorm column statistics of :115 fused into the epilogue,
  * their input / weight gradients, and the MoCo logits q.queue^T (gcc/contrastive/memory_moco.py:33-44).

@@ -8,7 +8,8 @@
  *
  * PARITY STATUS: "parity unpinned" against DGL.  The arithmetic of these
  * functions lives in DGL 0.4.3 (dgl.contrib.sampling.random_walk_with_restart,
- * DGLGraph.subgraph), which is absent from /root/reference and from this image
+ * DGLGraph.subgraph), which is not part of the reference and was not installable
+ * where this oracle was written
  * (SURVEY.md section 8c).  What IS followed line by line is the reference's own
  * glue around those calls:
  *   - seed draw p ~ in_deg^0.75         gcc/datasets/graph_dataset.py:85-92

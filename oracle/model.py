@@ -65,7 +65,7 @@ def _bn(x, params, key, train, stats_out, momentum=0.1, eps=1e-5):
 
 
 def _round_operand(x, dt):
-    """Round a GEMM operand to `dt` (bf16: what the tensor-core path feeds tcgen05) in the forward only
+    """Round a GEMM operand to `dt` (bf16: what the tensor-core path feeds wgmma) in the forward only
     (straight-through for autograd); accumulation stays in the oracle's precision."""
     if dt is None:
         return x

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Developer tool: build a differently-tuned libgccb200 (extra -D flags) into build_variants/ for
-A/B runs on the GPU box:  GCCB200_LIB=build_variants/libgccb200_NAME.so python bench.py ..."""
+A/B runs on the GPU:  GCCB200_LIB=build_variants/libgccb200_NAME.so python bench.py ..."""
 import glob
 import os
 import subprocess

@@ -1,6 +1,7 @@
 # GPU: spectral parity of the cluster path on explicit huge ego-nets (n = 520, 1500, 3300)
-import sys, ctypes as C, numpy as np, torch
-sys.path.insert(0, '/root/repo'); sys.path.insert(0, '/root/repo/tests')
+import os, sys, ctypes as C, numpy as np, torch
+_ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, _ROOT); sys.path.insert(0, os.path.join(_ROOT, 'tests'))
 from gcc_b200 import _lib
 from gcc_b200.datasets import synthetic
 from gcc_b200.datasets.graph_dataset import BatchBuffers

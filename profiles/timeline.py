@@ -1,9 +1,10 @@
 #!/usr/bin/env python
 """GPU diagnostic: CUPTI kernel timeline (torch.profiler) of a few pipelined engine steps.
-Writes gpurun_out/timeline.json.gz (chrome trace).  Diagnostic only -- never a bench value."""
+Writes a chrome trace to argv[2] (default: timeline.json.gz in the temporary directory).  Diagnostic only -- never a bench value."""
 import contextlib
 import os
 import sys
+import tempfile
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import gcc_b200  # noqa: F401  (sets CUDA_DEVICE_MAX_CONNECTIONS before CUDA starts)
@@ -41,6 +42,6 @@ with profile(activities=[ProfilerActivity.CUDA]) as prof:
     for _ in range(6):
         eng.step(lr=0.005)
     torch.cuda.synchronize()
-out = sys.argv[2] if len(sys.argv) > 2 else "gpurun_out/timeline.json.gz"
+out = sys.argv[2] if len(sys.argv) > 2 else os.path.join(tempfile.gettempdir(), "timeline.json.gz")
 prof.export_chrome_trace(out)
 print("wrote", out)

@@ -10,7 +10,7 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 CSRC = os.path.join(ROOT, "gcc_b200", "csrc")
 OUT = os.path.join(HERE, "_build")
 LIB = os.path.join(OUT, "libgccb200_emu.so")
-# kernels that need real sm_100a hardware features (tcgen05/TMA) are excluded
+# kernels that need real sm_90a hardware features (wgmma/TMA) are excluded
 EXCLUDE = {"tc_gemm.cu"}
 
 

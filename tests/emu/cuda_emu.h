@@ -6,7 +6,7 @@
 // in a container without a GPU.  Each CUDA thread of a block is a ucontext
 // fiber; blocks run one after another; __syncthreads()/warp collectives yield
 // to a round-robin scheduler.  It proves nothing about performance, memory
-// coalescing or data races -- the `-m gpu` parity tests on a real B200 do that.
+// coalescing or data races -- the `-m gpu` parity tests on a real H100 do that.
 // The product build (nvcc, libgccb200.so) never includes this header, and the
 // Python package cannot load the emulated library.
 #pragma once

@@ -1,6 +1,6 @@
 """A minimal stand-in for DGL 0.4.3, used ONLY by tests/golden/make_golden.py to
-execute the REAL reference modules (/root/reference/gcc/**, train.py) in this
-container, where DGL is absent and not installable (SURVEY.md section 8c).
+execute the REAL reference modules (gcc/**, train.py of a reference checkout)
+without DGL, which was not installable there (SURVEY.md section 8c).
 
 Everything here encodes the [M] (recalled, unverifiable) DGL semantics the
 oracle documents; everything *outside* this file that runs during golden

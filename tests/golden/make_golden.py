@@ -1,15 +1,15 @@
 #!/usr/bin/env python
 """Generate the golden fixtures in tests/golden/*.npz by executing the REAL
-reference modules from /root/reference (read-only) in THIS container.
+reference modules from a checkout of THUDM/GCC (read-only).
 
-DGL is absent here, so `dgl_stub.py` supplies the few DGL objects the hot path
+DGL 0.4.3 could not be installed where the fixtures were made, so `dgl_stub.py` supplies the few DGL objects the hot path
 touches (documented [M] semantics); every other line that runs is the
 reference's own: gcc.contrastive.{memory_moco,criterions}, gcc.utils.misc,
 gcc.models.{graph_encoder,gin}, gcc.datasets.{graph_dataset,data_util} and
 train.py's train_moco / moment_update / clip_grad_norm / train_finetune / test_finetune.
 
-Run:  python tests/golden/make_golden.py          (needs /root/reference)
-The fixtures are committed; the GPU box never needs /root/reference.
+Run:  GCC_REFERENCE=<checkout of THUDM/GCC> python tests/golden/make_golden.py
+The fixtures are committed; the tests never need the reference.
 """
 import argparse
 import os
@@ -23,7 +23,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, HERE)
-REF = os.environ.get("GCC_REFERENCE", "/root/reference")
+REF = os.environ.get("GCC_REFERENCE")
+if not REF or not os.path.isdir(REF):
+    raise SystemExit("set GCC_REFERENCE to a checkout of THUDM/GCC")
 
 import dgl_stub  # noqa: E402
 

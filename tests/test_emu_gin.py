@@ -1,6 +1,6 @@
 """CPU: GIN forward / backward, MoCo head and optimiser kernels under the fiber emulator
 versus the torch-CPU oracle (which tests/test_oracle_golden.py pins to the real reference).
-Kernel LOGIC only; the parity gate proper is tests/test_gpu_*.py on a B200."""
+Kernel LOGIC only; the parity gate proper is tests/test_gpu_*.py on an H100."""
 import ctypes as C
 
 import numpy as np

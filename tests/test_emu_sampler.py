@@ -1,6 +1,6 @@
 """CPU: sampler kernels (gcc_b200/csrc/sampler.cu) run under the fiber emulator and
 compared bit-for-bit with the oracle.  Kernel LOGIC only -- the real parity gate is
-tests/test_gpu_*.py on a B200."""
+tests/test_gpu_*.py on an H100."""
 import ctypes as C
 
 import numpy as np

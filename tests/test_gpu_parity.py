@@ -1,4 +1,4 @@
-"""GPU parity tests (B200): every kernel family of libgccb200, driven through the product's
+"""GPU parity tests (H100): every kernel family of libgccb200, driven through the product's
 Python API (which calls the C ABI), against the CPU oracle and the golden fixtures produced by
 the real reference modules.  Integer outputs must be bit-exact; floating point within the
 stated tolerances (north_star: 1e-3 relative for embeddings and loss)."""

@@ -272,7 +272,7 @@ def test_fused_infonce_real_sizes(B, K, d):
     _lib.check(lib.gccb_infonce_fused(_lib.dptr(q), _lib.dptr(k), _lib.dptr(mem), B, d, K, 0.07, _lib.dptr(stats),
                                       _lib.dptr(dq), _lib.dptr(ws), ws.numel(), _lib.stream_ptr()))
     torch.cuda.synchronize()
-    tc = d >= 128 and B >= 128 and os.environ.get("GCCB200_TC", "1") != "0"      # tcgen05 path (moco.cu: nce_use_tc)
+    tc = d >= 128 and B >= 128 and os.environ.get("GCCB200_TC", "1") != "0"      # tensor-core path (moco.cu: nce_use_tc)
     q64 = q.double().requires_grad_(True)
     # tensor-core path: the two big products take bf16 operands -> the oracle rounds q / queue the same way for the
     # negatives (the positive logit stays fp32 in the kernel)
@@ -328,12 +328,12 @@ def test_gin_wide_forward_backward_vs_oracle(H, tc):
     """BASELINE config 4 width: GraphEncoder(hidden 256 / 128, 5 layers) forward + backward through the module
     API against the torch-CPU float64 oracle with autograd.
       tc = 0: fp32 SIMT kernels vs the plain oracle: embeddings <= 1e-3, gradients <= 5e-3 of their scale.
-      tc = 1: tcgen05 path (bf16 operands, fp32 accumulation in TMEM) vs the oracle with ITS GEMM operands rounded
+      tc = 1: wgmma path (bf16 operands, fp32 accumulation in registers) vs the oracle with ITS GEMM operands rounded
               to bf16 the same way: embeddings <= 2e-3 (rms 3e-4) of the (unit) row norm -- what is left is the tensor core's
               forward rounding-boundary flips (an fp32 vs fp64 operand landing on the other side of a bf16
               boundary) through 8 chained GEMMs + BatchNorms.  Gradients: this BatchNorm/ReLU stack is very
               sensitive to operand rounding -- the ORACLE's own gradients move by 10-35% of their scale when its
-              operands are rounded to bf16 (measured, profiles/README.md) -- so the bar for the tensor-core
+              operands are rounded to bf16 (profiles/wide_grad_check.py measures it) -- so the bar for the tensor-core
               backward (which also rounds dz) is statistical: per weight tensor relative L2 error <= 8e-2 and
               cosine >= 0.995 against the bf16-operand oracle.
     fp32 (tc = 0) gradients are compared elementwise, allowing isolated ReLU-kink flips (one pre-activation within

@@ -1,4 +1,4 @@
-"""GPU (B200): the tcgen05 / TMEM / TMA contraction kernel (csrc/tc_gemm.cu) through the C ABI against
+"""GPU (H100): the wgmma / TMA contraction kernel (csrc/tc_gemm.cu) through the C ABI against
 torch fp32 matmul of the same bf16-rounded operands (fp32 accumulate on both sides: the only difference
 is summation order, so the bar is 2e-3 of the output scale)."""
 import numpy as np

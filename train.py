@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Pretraining driver with the reference's command line (THUDM/GCC train.py:40-130, pretraining
-flags only) on the B200-native hot path.
+flags only) on the H100-native hot path.
 
     python train.py --moco --nce-k 16384 --dataset synthetic-chunglu --graph-nodes 1000000 \
         --graph-edges 20000000 --batch-size 256 --epochs 1 --num-samples 2000 --num-workers 12
