@@ -41,6 +41,14 @@ class GinLayout(C.Structure):
                  "wp", "bp")] + [("emb", C.c_int64), ("total", C.c_int64), ("run_total", C.c_int64)]
 
 
+class GinStash(C.Structure):
+    _fields_ = ([("x0", C.c_int64)] + [(n, C.c_int64 * 8) for n in ("a", "z1", "z2", "h")] +
+                [("stats", C.c_int64), ("pooled", C.c_int64), ("a16", C.c_int64), ("x16", C.c_int64),
+                 ("w16", C.c_int64 * 8), ("dh", C.c_int64), ("g1", C.c_int64 * 2), ("dz2", C.c_int64 * 2)] +
+                [(n, C.c_int64) for n in ("da", "dpool", "coef1", "dz16", "tA", "tB")] +
+                [(n, C.c_int32) for n in ("cap_pad", "splits", "DW", "PW")])
+
+
 _PROTOS = {
     "gccb_version": (C.c_int, []),
     "gccb_arch": (C.c_int, []),
@@ -59,6 +67,7 @@ _PROTOS = {
     "gccb_gin_backward_workspace": (C.c_size_t, [C.POINTER(GinCfg), C.c_int32, C.c_int32]),
     "gccb_gin_backward": (C.c_int, [C.POINTER(GinCfg), C.POINTER(Batch), C.c_int32, p, p, p, p,
                                     C.c_uint64, C.c_uint64, C.c_int32, p, C.c_size_t, p]),
+    "gccb_gin_stash_layout": (C.c_int, [C.POINTER(GinCfg), C.c_int32, C.c_int32, C.POINTER(GinStash)]),
     "gccb_moco_logits": (C.c_int, [p, p, p, C.c_int32, C.c_int32, C.c_int32, C.c_float, p, p]),
     "gccb_moco_logits_backward": (C.c_int, [p, p, p, C.c_int32, C.c_int32, C.c_int32, C.c_float,
                                             p, p]),

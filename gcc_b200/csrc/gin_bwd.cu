@@ -17,52 +17,6 @@
 
 namespace gccb {
 
-#define GCCB_WG_CHUNKS GCCB_NUM_SMS    // row chunks of the weight-gradient split-K
-
-struct BwdLayout {            // byte offsets in the backward workspace
-  size_t dh, g1[2], dz2[2], da, red, dS, dpool, part, total;   // g1/dz2 alternate between layers
-  // tensor-core path: bf16 operand of the input-gradient GEMMs, two transposed bf16 operands of the weight-
-  // gradient GEMMs ([W][cap_pad]), per-layer BatchNorm-1 coefficients (sc | sh) and the split-K partials
-  size_t dz16, tA, tB, coef1, splitk;
-  int DW;                     // width of dh / da rows = max(H, 64)
-  int cap_pad, splits;
-};
-
-inline BwdLayout make_bwd_layout(const GinDims& d, int B, int node_cap) {
-  BwdLayout b;
-  size_t off = 0;
-  auto take = [&](size_t bytes) { size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
-  b.DW = d.H > GCCB_DINP ? d.H : GCCB_DINP;
-  b.dh = take((size_t)node_cap * b.DW * 4);
-  for (int i = 0; i < 2; ++i) {
-    b.g1[i] = take((size_t)node_cap * d.H * 4);
-    b.dz2[i] = take((size_t)node_cap * d.H * 4);
-  }
-  b.da = take((size_t)node_cap * b.DW * 4);
-  b.red = take((size_t)(d.L - 1) * 3 * 2 * d.H * 8);
-  b.dS = take((size_t)d.L * B * d.H * 4);
-  b.dpool = take((size_t)d.L * B * b.DW * 4);
-  b.part = take((size_t)GCCB_WG_CHUNKS * ((size_t)d.H * b.DW + d.H) * 4);
-  b.dz16 = b.tA = b.tB = b.coef1 = b.splitk = 0;
-  b.cap_pad = (node_cap + 63) & ~63;
-  b.splits = 0;
-#ifndef GCCB_EMU
-  if (d.tc) {
-    b.dz16 = take((size_t)node_cap * d.H * 2);
-    b.tA = take((size_t)d.H * b.cap_pad * 2);
-    b.tB = take((size_t)b.DW * b.cap_pad * 2);
-    b.coef1 = take((size_t)(d.L - 1) * 2 * d.H * 4);
-    const int tiles = (d.H / 128) * 1;                      // 128-row output tiles of a [H x <=256] weight gradient
-    b.splits = GCCB_NUM_SMS / tiles;
-    if (b.splits > b.cap_pad / 64) b.splits = b.cap_pad / 64;
-    if (b.splits < 1) b.splits = 1;
-    b.splitk = take((size_t)b.splits * d.H * b.DW * 4);
-  }
-#endif
-  b.total = off;
-  return b;
-}
-
 // ---- prediction heads + normalisation backward (one CTA per graph) ------------------------
 template <int H>
 __global__ void __launch_bounds__(256)
@@ -1103,6 +1057,49 @@ extern "C" size_t gccb_gin_backward_workspace(const gccb_gin_cfg_t* cfg, int32_t
   GinDims d;
   if (dims_from_cfg(cfg, &d)) return 0;
   return make_bwd_layout(d, batch, node_cap).total;
+}
+
+extern "C" int gccb_gin_stash_layout(const gccb_gin_cfg_t* cfg, int32_t batch, int32_t node_cap,
+                                     gccb_gin_stash_t* out) {
+  GinDims d;
+  int rc = dims_from_cfg(cfg, &d);
+  if (rc) return rc;
+  if (!out || batch < 1 || node_cap < 1) {
+    set_last_error("gccb_gin_stash_layout: bad argument");
+    return GCCB_ERR_BADARG;
+  }
+  const ActsLayout al = make_acts_layout(d, batch, node_cap);
+  const BwdLayout bl = make_bwd_layout(d, batch, node_cap);
+  auto tc = [&](size_t off) { return d.tc ? (int64_t)off : (int64_t)-1; };
+  out->x0 = (int64_t)al.x0;
+  for (int l = 0; l < 8; ++l) {
+    const bool live = l < d.L - 1;
+    out->a[l] = live ? (int64_t)al.a[l] : -1;
+    out->z1[l] = live ? (int64_t)al.z1[l] : -1;
+    out->z2[l] = live ? (int64_t)al.z2[l] : -1;
+    out->h[l] = live ? (int64_t)al.h[l] : -1;
+    out->w16[l] = live ? tc(al.w16[l]) : -1;
+  }
+  out->stats = (int64_t)al.stats;
+  out->pooled = (int64_t)al.pooled;
+  out->a16 = tc(al.a16);
+  out->x16 = tc(al.x16);
+  out->dh = (int64_t)bl.dh;
+  for (int i = 0; i < 2; ++i) {
+    out->g1[i] = (int64_t)bl.g1[i];
+    out->dz2[i] = (int64_t)bl.dz2[i];
+  }
+  out->da = (int64_t)bl.da;
+  out->dpool = (int64_t)bl.dpool;
+  out->coef1 = tc(bl.coef1);
+  out->dz16 = tc(bl.dz16);
+  out->tA = tc(bl.tA);
+  out->tB = tc(bl.tB);
+  out->cap_pad = d.tc ? bl.cap_pad : -1;
+  out->splits = d.tc ? bl.splits : -1;
+  out->DW = bl.DW;
+  out->PW = al.PW;
+  return GCCB_OK;
 }
 
 extern "C" int gccb_gin_backward(const gccb_gin_cfg_t* cfg, const gccb_batch_t* batch, int32_t view,

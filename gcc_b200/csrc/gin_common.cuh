@@ -68,6 +68,52 @@ inline ActsLayout make_acts_layout(const GinDims& d, int B, int node_cap) {
   return a;
 }
 
+#define GCCB_WG_CHUNKS GCCB_NUM_SMS    // row chunks of the weight-gradient split-K (SIMT backward)
+
+struct BwdLayout {            // byte offsets in the backward workspace
+  size_t dh, g1[2], dz2[2], da, red, dS, dpool, part, total;   // g1/dz2 alternate between layers
+  // tensor-core path: bf16 operand of the input-gradient GEMMs, two transposed bf16 operands of the weight-
+  // gradient GEMMs ([W][cap_pad]), per-layer BatchNorm-1 coefficients (sc | sh) and the split-K partials
+  size_t dz16, tA, tB, coef1, splitk;
+  int DW;                     // width of dh / da rows = max(H, 64)
+  int cap_pad, splits;
+};
+
+inline BwdLayout make_bwd_layout(const GinDims& d, int B, int node_cap) {
+  BwdLayout b;
+  size_t off = 0;
+  auto take = [&](size_t bytes) { size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
+  b.DW = d.H > GCCB_DINP ? d.H : GCCB_DINP;
+  b.dh = take((size_t)node_cap * b.DW * 4);
+  for (int i = 0; i < 2; ++i) {
+    b.g1[i] = take((size_t)node_cap * d.H * 4);
+    b.dz2[i] = take((size_t)node_cap * d.H * 4);
+  }
+  b.da = take((size_t)node_cap * b.DW * 4);
+  b.red = take((size_t)(d.L - 1) * 3 * 2 * d.H * 8);
+  b.dS = take((size_t)d.L * B * d.H * 4);
+  b.dpool = take((size_t)d.L * B * b.DW * 4);
+  b.part = take((size_t)GCCB_WG_CHUNKS * ((size_t)d.H * b.DW + d.H) * 4);
+  b.dz16 = b.tA = b.tB = b.coef1 = b.splitk = 0;
+  b.cap_pad = (node_cap + 63) & ~63;
+  b.splits = 0;
+#ifndef GCCB_EMU
+  if (d.tc) {
+    b.dz16 = take((size_t)node_cap * d.H * 2);
+    b.tA = take((size_t)d.H * b.cap_pad * 2);
+    b.tB = take((size_t)b.DW * b.cap_pad * 2);
+    b.coef1 = take((size_t)(d.L - 1) * 2 * d.H * 4);
+    const int tiles = (d.H / 128) * 1;                      // 128-row output tiles of a [H x <=256] weight gradient
+    b.splits = GCCB_NUM_SMS / tiles;
+    if (b.splits > b.cap_pad / 64) b.splits = b.cap_pad / 64;
+    if (b.splits < 1) b.splits = 1;
+    b.splitk = take((size_t)b.splits * d.H * b.DW * 4);
+  }
+#endif
+  b.total = off;
+  return b;
+}
+
 // flat parameter layout (floats); mirrors gccb_gin_layout_t
 inline void make_param_layout(const GinDims& d, gccb_gin_layout_t* o) {
   int64_t off = 0;

@@ -180,6 +180,26 @@ int gccb_gin_backward(const gccb_gin_cfg_t* cfg, const gccb_batch_t* batch, int3
                       uint64_t dropout_key, uint64_t dropout_step, int32_t dropout_layer_base,
                       void* workspace, size_t workspace_bytes, gccb_stream_t stream);
 
+/* Where the intermediates live, for tests and diagnostics (host-only query, no device work).
+ * Forward fields: byte offsets into the activation stash of gccb_gin_forward (x0 float [node_cap][64];
+ * a[l] float [node_cap][64 (l = 0) or hidden]; z1/z2/h[l] float [node_cap][hidden]; stats double
+ * [L-1][3][2][hidden]; pooled float [L][B][PW]; a16 bf16 = a of the last layer run; x16 bf16 = its
+ * relu(bn1(z1)); w16[l] bf16 W1 [hidden][KW] | W2 | W1^T [KW][hidden] | W2^T, KW = 64 (l = 0) or hidden).
+ * Backward fields: byte offsets into the workspace of gccb_gin_backward (dh, da float [node_cap][DW];
+ * g1/dz2[l & 1] float [node_cap][hidden], g1 ends as dz1; dpool float [L][B][DW]; coef1 float
+ * [L-1][sc | sh][hidden]; dz16 bf16 [node_cap][hidden]; tA bf16 [hidden][cap_pad], tB bf16 [DW][cap_pad]).
+ * A field the configuration does not have is -1 (every tensor-core field when cfg selects the fp32 path). */
+typedef struct {
+  int64_t x0, a[8], z1[8], z2[8], h[8], stats, pooled, a16, x16, w16[8];
+  int64_t dh, g1[2], dz2[2], da, dpool, coef1, dz16, tA, tB;
+  int32_t cap_pad;   /* rows of the transposed weight-gradient operands (node_cap rounded up to 64) */
+  int32_t splits;    /* split-K partitions of the weight-gradient GEMMs                            */
+  int32_t DW;        /* row width of dh / da / dpool = max(hidden, 64)                             */
+  int32_t PW;        /* row width of pooled = max(hidden, 64)                                      */
+} gccb_gin_stash_t;
+int gccb_gin_stash_layout(const gccb_gin_cfg_t* cfg, int32_t batch, int32_t node_cap,
+                          gccb_gin_stash_t* out /* host */);
+
 /* ---- contrastive head ------------------------------------------------------------------ */
 /* MemoryMoCo.forward logits (memory_moco.py:33-44): out[B][K+1] = [q.k | q.memory^T] / T */
 int gccb_moco_logits(const float* q, const float* k, const float* memory, int32_t B,

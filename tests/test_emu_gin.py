@@ -8,6 +8,7 @@ import pytest
 import torch
 
 from emu_util import NpBatch, lib, ptr
+from gcc_b200 import _capi
 from gcc_b200.datasets import synthetic
 from gcc_b200.models import layout as glayout
 from oracle import model as om
@@ -124,6 +125,49 @@ def test_gin_forward_backward_vs_oracle(L, H, B_, hops):
     # running statistics: both forwards updated the same buffers (two train-mode passes)
     assert np.all(nbt == 2)
     assert not np.allclose(running, running0)
+
+
+def test_stash_layout_locates_the_forward_intermediates(monkeypatch):
+    """gccb_gin_stash_layout: the emulator build has no tensor-core path, so every tensor-core field is -1 even
+    when the configuration asks for tensor cores; the offsets it reports for z1, z2 and h of a layer hold what
+    the oracle computes there."""
+    Lb = lib()
+    L, H = 3, 32
+    b, views, pos = _batch(4, 12)
+    for tc_cfg in (glayout.make_cfg(num_layers=4, hidden=128, tensor_cores=1), glayout.make_cfg(num_layers=L, hidden=H)):
+        st = _capi.GinStash()
+        assert Lb.gccb_gin_stash_layout(C.byref(tc_cfg), b.B, b.node_cap, C.byref(st)) == 0, Lb.gccb_last_error()
+        for name in ("a16", "x16", "coef1", "dz16", "tA", "tB", "cap_pad", "splits"):
+            assert getattr(st, name) == -1, name
+        assert list(st.w16) == [-1] * 8
+        nl = tc_cfg.num_layers - 1
+        assert all(x >= 0 for x in list(st.z1)[:nl]) and list(st.z1)[nl:] == [-1] * (8 - nl)
+        assert st.DW == st.PW == max(tc_cfg.hidden, 64) and st.dz2[1] > st.dz2[0] >= 0
+    cfg = glayout.make_cfg(num_layers=L, hidden=H)
+    flat, sd, _ = _params(cfg, np.random.default_rng(9))
+    running = np.zeros(glayout.running_slices(cfg)[1], np.float32)
+    acts = np.zeros(Lb.gccb_gin_acts_bytes(C.byref(cfg), b.B, b.node_cap), np.uint8)
+    feat = np.zeros((b.B, H), np.float32)
+    rc = Lb.gccb_gin_forward(C.byref(cfg), C.byref(b.c), 0, ptr(pos), ptr(flat), ptr(running), None, 1, 0, 0, -1,
+                             ptr(acts), acts.nbytes, ptr(feat), None, None)
+    assert rc == 0, Lb.gccb_last_error()
+    ov = _oracle_view(b, views, pos, 0)
+    seen = []                                    # per GIN layer the oracle normalises z1, z2, then y = relu(bn_a(z2))
+    bn = om._bn
+
+    def record(x, *a, **k):
+        y = bn(x, *a, **k)
+        seen.append((x.detach(), y.detach()))
+        return y
+    monkeypatch.setattr(om, "_bn", record)
+    om.gin_encoder_forward(sd, ov["indptr"], ov["indices"], torch.from_numpy(ov["pos"]).double(), ov["seed"],
+                           ov["sub_deg"], ov["node_off"], num_layers=L)
+    N, l = int(b.node_off[0, b.B]), 1
+    for got_off, want in ((st.z1[l], seen[3 * l][0]), (st.z2[l], seen[3 * l + 1][0]),
+                          (st.h[l], torch.relu(seen[3 * l + 2][1]))):
+        got = acts[got_off:got_off + N * H * 4].view(np.float32).reshape(N, H)
+        assert np.allclose(got, want.numpy(), rtol=1e-4, atol=1e-4 * float(want.abs().max())), \
+            np.abs(got - want.numpy()).max()
 
 
 def test_moco_head_and_optimiser_vs_oracle():
