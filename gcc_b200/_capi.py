@@ -80,6 +80,10 @@ _PROTOS = {
     "gccb_clip_adam_ema": (C.c_int, [p, p, p, p, p, C.c_int64, C.c_int64, p, C.c_float,
                                      C.c_float, C.c_float, C.c_float, C.c_float, C.c_float,
                                      C.c_float, p, p, p, C.c_int32, p]),
+    "gccb_clip_sgd_ema": (C.c_int, [p, p, p, p, C.c_int64, C.c_int64, p, C.c_float, C.c_float, C.c_float,
+                                    C.c_float, C.c_float, p, p, p, C.c_int32, p]),
+    "gccb_clip_adagrad_ema": (C.c_int, [p, p, p, p, C.c_int64, C.c_int64, p, C.c_float, C.c_float, C.c_float,
+                                        C.c_float, C.c_float, p, p, p, C.c_int32, p]),
     "gccb_sum_ranks": (C.c_int, [p, C.c_int32, C.c_int64, C.c_int64, p, C.c_int64, p, p]),
     "gccb_tc_gemm_bf16": (C.c_int, [p, p, C.c_int32, C.c_int32, C.c_int32, p, p, C.c_float, p, p, C.c_int32, p,
                                     C.c_int32, p, p]),

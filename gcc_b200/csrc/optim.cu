@@ -1,8 +1,8 @@
-// optim.cu -- gradient clipping, Adam and the momentum-encoder update on flat buffers.
+// optim.cu -- gradient clipping, the optimiser step and the momentum-encoder update on flat buffers.
 //
 // Replaces (reference file:line):
 //   clip_grad_norm -> torch.nn.utils.clip_grad_norm_(params, 1.0)     train.py:340-347,409
-//   torch.optim.Adam(lr, betas, weight_decay = L2 added to the grad)  train.py:417,667-672
+//   torch.optim.{SGD,Adam,Adagrad}(lr, ..., weight_decay = L2 added to the grad)  train.py:417,659-678
 //   moment_update: p_ema = m p_ema + (1-m) p over model.parameters()  train.py:169-172,430-431
 // The reference launches 51 + 2*67 tiny per-tensor kernels; here all live parameters are one
 // flat buffer (gccb_gin_layout_t), so a step is one reduction and one elementwise kernel.
@@ -28,15 +28,73 @@ gradnorm_kernel(const float* __restrict__ g, int64_t n, float scale, double* __r
   }
 }
 
-// hyper: [0] lr, [1] 1 - beta1^t, [2] sqrt(1 - beta2^t)
+// Update rules of clip_update_ema_kernel.  load() reads the step's scalars from the device `hyper` array;
+// apply() takes a live entry's parameter pv and its clipped, weight-decayed gradient d, updates the rule's
+// per-entry state (s0, s1) and returns the new parameter.  Each restates its torch.optim.*.step (torch 2.x,
+// single-tensor path) for one fp32 entry.
+
+// torch.optim.Adam (train.py:667-672).  hyper: [0] lr, [1] 1 - beta1^t, [2] sqrt(1 - beta2^t).
+// s0 = exp_avg, s1 = exp_avg_sq.
+struct AdamRule {
+  float beta1, beta2, eps;
+  float lr, bc1, sbc2;
+  __device__ __forceinline__ void load(const float* __restrict__ hyper) {
+    lr = hyper[0];
+    bc1 = hyper[1];
+    sbc2 = hyper[2];
+  }
+  __device__ __forceinline__ float apply(int64_t i, float pv, float d, float* __restrict__ m,
+                                         float* __restrict__ v) const {
+    float mv = beta1 * m[i] + (1.0f - beta1) * d;
+    float vv = beta2 * v[i] + (1.0f - beta2) * d * d;
+    m[i] = mv;
+    v[i] = vv;
+    float denom = sqrtf(vv) / sbc2 + eps;
+    return pv - (lr / bc1) * (mv / denom);
+  }
+};
+
+// torch.optim.SGD with dampening 0 and no Nesterov (train.py:660-665).  hyper: [0] lr.  s0 = momentum_buffer,
+// untouched (and may be null) when momentum == 0.
+struct SgdRule {
+  float momentum;
+  float lr;
+  __device__ __forceinline__ void load(const float* __restrict__ hyper) { lr = hyper[0]; }
+  __device__ __forceinline__ float apply(int64_t i, float pv, float d, float* __restrict__ buf,
+                                         float* __restrict__) const {
+    if (momentum != 0.f) {
+      // torch starts the buffer as a copy of d on the first step.  With dampening 0, a buffer that starts
+      // at zero gives momentum * 0 + d = d, the same value, so the kernel needs no first-step branch.
+      d = momentum * buf[i] + d;
+      buf[i] = d;
+    }
+    return pv - lr * d;
+  }
+};
+
+// torch.optim.Adagrad with initial_accumulator_value 0 (train.py:674-678).  hyper: [0] clr =
+// lr / (1 + (t - 1) * lr_decay), computed in double on the host.  s0 = sum.
+struct AdagradRule {
+  float eps;
+  float clr;
+  __device__ __forceinline__ void load(const float* __restrict__ hyper) { clr = hyper[0]; }
+  __device__ __forceinline__ float apply(int64_t i, float pv, float d, float* __restrict__ sum,
+                                         float* __restrict__) const {
+    float s = sum[i] + d * d;
+    sum[i] = s;
+    return pv - clr * (d / (sqrtf(s) + eps));
+  }
+};
+
+template <class Rule>
 __global__ void __launch_bounds__(256)
-adam_ema_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
-                float* __restrict__ v, float* __restrict__ p_ema, int64_t n_live, int64_t n_all,
-                const float* __restrict__ hyper, float beta1, float beta2, float eps, float wd,
-                float clip_norm, float alpha, float grad_scale, const double* __restrict__ sumsq,
-                float* __restrict__ grad_norm_out, const int32_t* __restrict__ skip_word, int32_t skip_mask) {
+clip_update_ema_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ s0,
+                       float* __restrict__ s1, float* __restrict__ p_ema, int64_t n_live, int64_t n_all,
+                       const float* __restrict__ hyper, Rule rule, float wd, float clip_norm, float alpha,
+                       float grad_scale, const double* __restrict__ sumsq, float* __restrict__ grad_norm_out,
+                       const int32_t* __restrict__ skip_word, int32_t skip_mask) {
   // a batch whose view was published empty (capacity overflow) must not move the weights: the whole
-  // update (Adam moments, parameters, momentum encoder) is a no-op for that step
+  // update (optimiser state, parameters, momentum encoder) is a no-op for that step
   if (skip_word && (*skip_word & skip_mask)) return;
   const float total = (float)sqrt(*sumsq);
   float coef = 1.0f;
@@ -44,19 +102,14 @@ adam_ema_kernel(float* __restrict__ p, const float* __restrict__ g, float* __res
     coef = clip_norm / (total + 1e-6f);
     if (coef > 1.0f) coef = 1.0f;
   }
-  const float lr = hyper[0], bc1 = hyper[1], sbc2 = hyper[2];
+  rule.load(hyper);
   if (blockIdx.x == 0 && threadIdx.x == 0 && grad_norm_out) *grad_norm_out = total;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_all; i += (int64_t)gridDim.x * blockDim.x) {
     float pv = p[i];
     if (i < n_live) {
       float gv = g[i] * grad_scale * coef;
       gv = fmaf(wd, pv, gv);                              // L2 weight decay folded into the gradient
-      float mv = beta1 * m[i] + (1.0f - beta1) * gv;
-      float vv = beta2 * v[i] + (1.0f - beta2) * gv * gv;
-      m[i] = mv;
-      v[i] = vv;
-      float denom = sqrtf(vv) / sbc2 + eps;
-      pv = pv - (lr / bc1) * (mv / denom);
+      pv = rule.apply(i, pv, gv, s0, s1);
       p[i] = pv;
     }
     if (alpha >= 0.f && p_ema) p_ema[i] = p_ema[i] * alpha + (1.0f - alpha) * pv;
@@ -82,6 +135,29 @@ sum_ranks_kernel(const float* __restrict__ gathered, int world, int64_t stride, 
 
 using namespace gccb;
 
+namespace {
+
+// The clip norm (gradnorm_kernel) then the update of every live entry and the EMA of all n_all entries
+// (clip_update_ema_kernel<Rule>), on `stream`.
+template <class Rule>
+int clip_update_ema(const char* name, float* p, const float* g, float* s0, float* s1, float* p_ema, int64_t n_live,
+                    int64_t n_all, const float* hyper, Rule rule, float weight_decay, float clip_norm, float alpha,
+                    float grad_scale, float* grad_norm_out, double* workspace, const int32_t* skip_word,
+                    int32_t skip_mask, gccb_stream_t stream) {
+  cudaMemsetAsync(workspace, 0, sizeof(double), (cudaStream_t)stream);
+  int blocks = (int)((n_live + 255) / 256);
+  if (blocks > 4 * GCCB_NUM_SMS) blocks = 4 * GCCB_NUM_SMS;
+  GCCB_LAUNCH(gradnorm_kernel, blocks, 256, 0, stream, g, n_live, grad_scale, workspace);
+  int blocks2 = (int)((n_all + 255) / 256);
+  if (blocks2 > 1184) blocks2 = 1184;
+  GCCB_LAUNCH(clip_update_ema_kernel<Rule>, blocks2, 256, 0, stream, p, g, s0, s1, p_ema, n_live, n_all, hyper,
+              rule, weight_decay, clip_norm, alpha, grad_scale, (const double*)workspace, grad_norm_out, skip_word,
+              skip_mask);
+  return check_launch(name);
+}
+
+}  // namespace
+
 extern "C" int gccb_clip_adam_ema(float* p, float* g, float* m, float* v, float* p_ema, int64_t n_live,
                                   int64_t n_all, const float* hyper, float beta1, float beta2, float eps,
                                   float weight_decay, float clip_norm, float alpha, float grad_scale,
@@ -91,16 +167,36 @@ extern "C" int gccb_clip_adam_ema(float* p, float* g, float* m, float* v, float*
     set_last_error("gccb_clip_adam_ema: bad argument");
     return GCCB_ERR_BADARG;
   }
-  cudaMemsetAsync(workspace, 0, sizeof(double), (cudaStream_t)stream);
-  int blocks = (int)((n_live + 255) / 256);
-  if (blocks > 4 * GCCB_NUM_SMS) blocks = 4 * GCCB_NUM_SMS;
-  GCCB_LAUNCH(gradnorm_kernel, blocks, 256, 0, stream, (const float*)g, n_live, grad_scale, workspace);
-  int blocks2 = (int)((n_all + 255) / 256);
-  if (blocks2 > 1184) blocks2 = 1184;
-  GCCB_LAUNCH(adam_ema_kernel, blocks2, 256, 0, stream, p, (const float*)g, m, v, p_ema, n_live, n_all, hyper,
-              beta1, beta2, eps, weight_decay, clip_norm, alpha, grad_scale, (const double*)workspace,
-              grad_norm_out, skip_word, skip_mask);
-  return check_launch("gccb_clip_adam_ema");
+  AdamRule rule{beta1, beta2, eps, 0.f, 0.f, 0.f};
+  return clip_update_ema("gccb_clip_adam_ema", p, g, m, v, p_ema, n_live, n_all, hyper, rule, weight_decay,
+                         clip_norm, alpha, grad_scale, grad_norm_out, workspace, skip_word, skip_mask, stream);
+}
+
+extern "C" int gccb_clip_sgd_ema(float* p, float* g, float* buf, float* p_ema, int64_t n_live, int64_t n_all,
+                                 const float* hyper, float momentum, float weight_decay, float clip_norm, float alpha,
+                                 float grad_scale, float* grad_norm_out, double* workspace, const int32_t* skip_word,
+                                 int32_t skip_mask, gccb_stream_t stream) {
+  if (!p || !g || (momentum != 0.f && !buf) || !hyper || !workspace || n_live <= 0 || n_all < n_live) {
+    set_last_error("gccb_clip_sgd_ema: bad argument");
+    return GCCB_ERR_BADARG;
+  }
+  SgdRule rule{momentum, 0.f};
+  return clip_update_ema("gccb_clip_sgd_ema", p, g, buf, nullptr, p_ema, n_live, n_all, hyper, rule, weight_decay,
+                         clip_norm, alpha, grad_scale, grad_norm_out, workspace, skip_word, skip_mask, stream);
+}
+
+extern "C" int gccb_clip_adagrad_ema(float* p, float* g, float* sum, float* p_ema, int64_t n_live, int64_t n_all,
+                                     const float* hyper, float eps, float weight_decay, float clip_norm, float alpha,
+                                     float grad_scale, float* grad_norm_out, double* workspace,
+                                     const int32_t* skip_word, int32_t skip_mask, gccb_stream_t stream) {
+  if (!p || !g || !sum || !hyper || !workspace || n_live <= 0 || n_all < n_live) {
+    set_last_error("gccb_clip_adagrad_ema: bad argument");
+    return GCCB_ERR_BADARG;
+  }
+  AdagradRule rule{eps, 0.f};
+  return clip_update_ema("gccb_clip_adagrad_ema", p, g, sum, nullptr, p_ema, n_live, n_all, hyper, rule,
+                         weight_decay, clip_norm, alpha, grad_scale, grad_norm_out, workspace, skip_word, skip_mask,
+                         stream);
 }
 
 extern "C" int gccb_sum_ranks(const float* gathered, int32_t world, int64_t stride, int64_t n, float* out,

@@ -5,7 +5,7 @@ feeds it) as a fixed sequence of libgccb200 kernel launches with no host synchro
   -> GIN forward q (model) and k (model_ema, BN in train mode, train.py:357-365)
   -> fused InfoNCE (loss, dq; logits never materialised)                     (memory_moco.py, criterions.py)
   -> GIN backward -> [all-gather of keys+grads when world > 1]
-  -> clip + Adam + momentum update on flat buffers (train.py:409-417,430-431)
+  -> clip + optimiser step (Adam, SGD or Adagrad) + momentum update on flat buffers (train.py:409-417,430-431)
   -> FIFO enqueue of the keys (memory_moco.py:55-61)
 
 The module-level API (GraphEncoder.forward + autograd, MemoryMoCo.forward, NCESoftmaxLoss) runs
@@ -22,17 +22,25 @@ from . import _capi, _lib
 from .datasets.data_util import BatchedSubgraphs
 from .parallel import StepExchange, first_sample_id
 
+ADAGRAD_EPS = 1e-10                                    # torch.optim.Adagrad's default; train.py never sets it
+
 
 class PretrainEngine:
     def __init__(self, dataset, model, model_ema, contrast, moco=True, learning_rate=0.005,
                  betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-5, clip_norm=1.0, alpha=0.999,
-                 nce_t=0.07, rank=0, world_size=1, process_group=None, prefetch=4):
+                 nce_t=0.07, rank=0, world_size=1, process_group=None, prefetch=4, optimizer="adam",
+                 momentum=0.9, lr_decay=0.0):
+        """optimizer: "adam" (betas, eps), "sgd" (momentum; dampening 0, no Nesterov) or "adagrad" (lr_decay;
+        eps 1e-10), as train.py:659-678 builds them over model.parameters()."""
+        if optimizer not in ("adam", "sgd", "adagrad"):
+            raise ValueError("optimizer must be adam, sgd or adagrad, not %r" % (optimizer,))
         _lib.require_device()
         self.lib = _lib.get()
         self.ds, self.model, self.model_ema, self.contrast = dataset, model, model_ema, contrast
         self.moco, self.lr0, self.betas, self.eps = moco, learning_rate, betas, eps
         self.wd, self.clip, self.alpha, self.T = weight_decay, clip_norm, alpha, nce_t
         self.rank, self.world, self.pg = rank, world_size, process_group
+        self.optimizer, self.momentum, self.lr_decay = optimizer, momentum, lr_decay
         dev = model.flat_params.device
         self.dev = dev
         B, H, L = dataset.batch_size, model.cfg.hidden, model.cfg.num_layers
@@ -46,9 +54,15 @@ class PretrainEngine:
             self.xch = StepExchange(B, H, n_live, world_size, dev, process_group)
             self.payload = self.xch.payload
         self.grads = self.xch.grads_send if self.xch else torch.zeros(n_live, **f32)
-        self.adam_m = torch.zeros(n_live, **f32)
-        self.adam_v = torch.zeros(n_live, **f32)
-        self.adam_t = 0
+        self.adam_m = self.adam_v = self.opt_state = None
+        if optimizer == "adam":
+            self.adam_m = torch.zeros(n_live, **f32)
+            self.adam_v = torch.zeros(n_live, **f32)
+        elif optimizer == "adagrad" or momentum != 0:
+            # SGD's momentum_buffer or Adagrad's sum over the live parameters; zero is also torch's starting
+            # point (Adagrad's initial_accumulator_value 0; SGD's first-step copy, see csrc/optim.cu)
+            self.opt_state = torch.zeros(n_live, **f32)
+        self.adam_t = 0                                # steps issued (skipped ones included), every optimiser
         self.hyper = torch.zeros(4, **f32)
         # ring of pinned slots: the host enqueues several steps ahead of the device, and an async H2D copy
         # reads its pinned source when it EXECUTES, so each step needs a slot of its own
@@ -114,11 +128,16 @@ class PretrainEngine:
 
     def _hyper(self, lr):
         self.adam_t += 1
-        b1, b2 = self.betas
         slot = self.hyper_host[self.adam_t % self.hyper_host.shape[0]]
-        slot[0] = lr
-        slot[1] = 1.0 - b1 ** self.adam_t
-        slot[2] = math.sqrt(1.0 - b2 ** self.adam_t)
+        if self.optimizer == "adam":
+            b1, b2 = self.betas
+            slot[0] = lr
+            slot[1] = 1.0 - b1 ** self.adam_t
+            slot[2] = math.sqrt(1.0 - b2 ** self.adam_t)
+        elif self.optimizer == "sgd":
+            slot[0] = lr
+        else:                                          # torch.optim.Adagrad's clr, in double
+            slot[0] = lr / (1.0 + (self.adam_t - 1) * self.lr_decay)
         self.hyper.copy_(slot, non_blocking=True)
 
     def _prepare(self, seeds):
@@ -235,7 +254,7 @@ class PretrainEngine:
             self.consumed[self.global_step % self.depth].record()
         grads, scale = self.grads, 1.0
         # a batch published empty (capacity overflow; the flag is raised for the host) must not train:
-        # Adam / EMA / enqueue skip the step on the device, the flags reach the host in read_stats()
+        # optimiser / EMA / enqueue skip the step on the device, the flags reach the host in read_stats()
         OVERFLOW = _capi.FLAG_NODE_OVERFLOW | _capi.FLAG_EDGE_OVERFLOW
         skip_word, skip_mask = _lib.dptr(buf.flags), OVERFLOW
         if self.world > 1:
@@ -249,15 +268,18 @@ class PretrainEngine:
             scale = 1.0 / self.world
             skip_word, skip_mask = _lib.dptr(self.any_skip), -1     # every replica skips the same steps
         self._hyper(lr)
-        _lib.check(lib.gccb_clip_adam_ema(_lib.dptr(model.flat_params), _lib.dptr(grads),
-                                          _lib.dptr(self.adam_m), _lib.dptr(self.adam_v),
-                                          _lib.dptr(ema.flat_params) if self.moco else None,
-                                          model.n_live, model._n_all, _lib.dptr(self.hyper), self.betas[0],
-                                          self.betas[1], self.eps, self.wd, self.clip,
-                                          self.alpha if self.moco else -1.0, scale,
-                                          C.c_void_p(self.stats.data_ptr() + 8), _lib.dptr(self.norm_ws),
-                                          skip_word, skip_mask, st),
-                   "gccb_clip_adam_ema")
+        p_ema, alpha = (_lib.dptr(ema.flat_params), self.alpha) if self.moco else (None, -1.0)
+        tail = (p_ema, model.n_live, model._n_all, _lib.dptr(self.hyper))
+        common = (self.wd, self.clip, alpha, scale, C.c_void_p(self.stats.data_ptr() + 8), _lib.dptr(self.norm_ws),
+                  skip_word, skip_mask, st)
+        p_, g_, s_ = _lib.dptr(model.flat_params), _lib.dptr(grads), _lib.dptr(self.opt_state)
+        if self.optimizer == "adam":
+            _lib.check(lib.gccb_clip_adam_ema(p_, g_, _lib.dptr(self.adam_m), _lib.dptr(self.adam_v), *tail,
+                                              self.betas[0], self.betas[1], self.eps, *common), "gccb_clip_adam_ema")
+        elif self.optimizer == "sgd":
+            _lib.check(lib.gccb_clip_sgd_ema(p_, g_, s_, *tail, self.momentum, *common), "gccb_clip_sgd_ema")
+        else:
+            _lib.check(lib.gccb_clip_adagrad_ema(p_, g_, s_, *tail, ADAGRAD_EPS, *common), "gccb_clip_adagrad_ema")
         if self.moco:
             # all ranks' keys in rank order with one launch -> identical queues on every rank
             src = self.xch.gathered if self.world > 1 else self.feat_k
@@ -301,22 +323,43 @@ class PretrainEngine:
                     window_prob=acc[1] / w, window_grad_norm=acc[2] / w)
 
     def optimizer_state_dict(self):
-        """The flat Adam buffers in the layout of torch.optim.Adam(model.parameters()).state_dict()
-        (train.py:667-672,752): per-parameter exp_avg / exp_avg_sq / step for the parameters that receive
+        """The flat optimiser buffers in the layout of torch.optim.{Adam,SGD,Adagrad}(model.parameters())
+        .state_dict() (train.py:659-678,752).  Adam: exp_avg / exp_avg_sq / step for the parameters that receive
         gradients (the GIN path); the unused set2set / lin_readout tensors have no state, as in the reference
-        where they never get a gradient."""
+        where they never get a gradient.  SGD: momentum_buffer for those parameters once a step has run, and
+        no state without momentum.  Adagrad: state for every parameter, as torch creates it at construction --
+        the unused tensors keep step 0 and a zero sum."""
         names = [n for n, _ in self.model.named_parameters()]
         state = {}
-        for i, n in enumerate(names):
+        for i, (n, prm) in enumerate(self.model.named_parameters()):
             if n in self.model._slices:
                 o, shape = self.model._slices[n]
                 cnt = 1
                 for d_ in shape:
                     cnt *= d_
-                state[i] = {"step": torch.tensor(float(self.adam_t)),
-                            "exp_avg": self.adam_m[o:o + cnt].view(shape).clone(),
-                            "exp_avg_sq": self.adam_v[o:o + cnt].view(shape).clone()}
-        group = {"lr": self.lr0, "betas": tuple(self.betas), "eps": self.eps, "weight_decay": self.wd,
-                 "amsgrad": False, "maximize": False, "foreach": None, "capturable": False, "differentiable": False,
-                 "fused": None, "params": list(range(len(names)))}
+                if self.optimizer == "adam":
+                    state[i] = {"step": torch.tensor(float(self.adam_t)),
+                                "exp_avg": self.adam_m[o:o + cnt].view(shape).clone(),
+                                "exp_avg_sq": self.adam_v[o:o + cnt].view(shape).clone()}
+                elif self.optimizer == "sgd":
+                    if self.opt_state is not None and self.adam_t > 0:
+                        state[i] = {"momentum_buffer": self.opt_state[o:o + cnt].view(shape).clone()}
+                else:
+                    state[i] = {"step": torch.tensor(float(self.adam_t)),
+                                "sum": self.opt_state[o:o + cnt].view(shape).clone()}
+            elif self.optimizer == "adagrad":
+                state[i] = {"step": torch.tensor(0.0), "sum": torch.zeros_like(prm.detach())}
+        params = list(range(len(names)))
+        if self.optimizer == "adam":
+            group = {"lr": self.lr0, "betas": tuple(self.betas), "eps": self.eps, "weight_decay": self.wd,
+                     "amsgrad": False, "maximize": False, "foreach": None, "capturable": False,
+                     "differentiable": False, "fused": None, "params": params}
+        elif self.optimizer == "sgd":
+            group = {"lr": self.lr0, "momentum": self.momentum, "dampening": 0, "weight_decay": self.wd,
+                     "nesterov": False, "maximize": False, "foreach": None, "differentiable": False, "fused": None,
+                     "params": params}
+        else:
+            group = {"lr": self.lr0, "lr_decay": self.lr_decay, "eps": ADAGRAD_EPS, "weight_decay": self.wd,
+                     "initial_accumulator_value": 0, "foreach": None, "maximize": False, "differentiable": False,
+                     "fused": None, "params": params}
         return {"state": state, "param_groups": [group]}

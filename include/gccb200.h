@@ -247,9 +247,25 @@ int gccb_clip_adam_ema(float* p, float* g, float* m, float* v, float* p_ema, int
                        float weight_decay, float clip_norm, float alpha, float grad_scale,
                        float* grad_norm_out, double* workspace /* 1 double */,
                        const int32_t* skip_word, int32_t skip_mask, gccb_stream_t stream);
+/* The same clip, EMA, grad_scale and skip word with torch.optim.SGD (dampening 0, no Nesterov;
+ * train.py:659-665) as the update: d = clipped g + weight_decay * p; buf = momentum * buf + d;
+ * p -= lr * buf.  buf (n_live floats) starts at zero, which equals torch's first-step copy of d.
+ * With momentum == 0 the update is p -= lr * d and buf may be NULL.  hyper[0] = lr.          */
+int gccb_clip_sgd_ema(float* p, float* g, float* buf, float* p_ema, int64_t n_live, int64_t n_all,
+                      const float* hyper, float momentum, float weight_decay, float clip_norm, float alpha,
+                      float grad_scale, float* grad_norm_out, double* workspace /* 1 double */,
+                      const int32_t* skip_word, int32_t skip_mask, gccb_stream_t stream);
+/* ... with torch.optim.Adagrad (initial_accumulator_value 0; train.py:673-678) as the update:
+ * sum += d * d; p -= clr * d / (sqrt(sum) + eps).  sum (n_live floats) starts at zero.
+ * hyper[0] = clr = lr / (1 + (t - 1) * lr_decay) for step t.                                  */
+int gccb_clip_adagrad_ema(float* p, float* g, float* sum, float* p_ema, int64_t n_live, int64_t n_all,
+                          const float* hyper, float eps, float weight_decay, float clip_norm, float alpha,
+                          float grad_scale, float* grad_norm_out, double* workspace /* 1 double */,
+                          const int32_t* skip_word, int32_t skip_mask, gccb_stream_t stream);
 /* deterministic rank-ordered sum of `world` gathered gradient buffers: out = sum_r in[r].
  * any_flag_out (optional, device int): set to 1 when gathered[r*stride + flag_index] != 0 for any
- * rank r (a rank whose batch overflowed), else 0 -- the skip word of the two calls above when
+ * rank r (a rank whose batch overflowed), else 0 -- the skip word of gccb_moco_enqueue and of the
+ * optimiser calls above when
  * world > 1, so that all replicas skip the same steps and stay identical.                    */
 int gccb_sum_ranks(const float* gathered, int32_t world, int64_t stride, int64_t n, float* out,
                    int64_t flag_index, int32_t* any_flag_out, gccb_stream_t stream);

@@ -10,8 +10,8 @@ What it keeps from the reference: flag names and defaults, run naming (train.py:
 triangular LR schedule with 10% warm-up (train.py:411-416, gcc/utils/misc.py:5-10), BatchNorm of the
 momentum encoder in train mode (train.py:357-365), the checkpoint dict
 {"opt","model","contrast","optimizer","epoch","model_ema"} with the reference's state_dict keys
-(train.py:748-786; "optimizer" is a torch.optim.Adam state_dict over model.parameters(), built from the
-flat Adam buffers), print/TensorBoard scalars (train.py:438-472), and the reference's step indexing:
+(train.py:748-786; "optimizer" is the state_dict of the torch.optim.SGD / Adam / Adagrad that --optimizer
+names, over model.parameters(), built from the flat optimiser buffers), print/TensorBoard scalars (train.py:438-472), and the reference's step indexing:
 epochs are 1-based and global_step = epoch * n_batch + idx (train.py:411,733), so the LR schedule starts
 one epoch into its warm-up exactly like the reference's.  What changes: the data loader and the whole
 step run on the GPU through gcc_b200.engine.PretrainEngine (no DataLoader workers, no .item() per step:
@@ -20,8 +20,8 @@ the meters average over all steps like the reference's).
 
 Fine-tuning (--finetune, train.py:175-337,516-545,631-660,788-792 of the reference): train_finetune /
 test_finetune keep the reference's signatures and arithmetic -- GraphEncoder forward/backward through the
-same device kernels (autograd Function), torch's Linear head, CrossEntropyLoss, clip_grad_value_(1), two
-torch Adam optimisers, micro-F1 per batch -- over the labeled datasets of gcc_b200/datasets/labeled.py,
+same device kernels (autograd Function), torch's Linear head, CrossEntropyLoss, clip_grad_value_(1), the
+--optimizer for the encoder and Adam for the output layer, micro-F1 per batch -- over the labeled datasets of gcc_b200/datasets/labeled.py,
 split by the reference's StratifiedKFold(10, shuffle, seed)[fold_idx].
 
     python train.py --finetune --dataset usa_airport --resume saved/.../current.pth --epochs 30 --fold-idx 0
@@ -53,11 +53,14 @@ def parse_option(argv=None):
     parser.add_argument("--num-samples", type=int, default=2000, help="num of samples per batch per worker")
     parser.add_argument("--epochs", type=int, default=100, help="number of training epochs")
     # optimization
-    parser.add_argument("--optimizer", type=str, default="adam", choices=["adam"], help="optimizer (flat Adam kernel)")
+    parser.add_argument("--optimizer", type=str, default="adam", choices=["sgd", "adam", "adagrad"], help="optimizer")
     parser.add_argument("--learning_rate", type=float, default=0.005, help="learning rate")
+    parser.add_argument("--lr_decay_epochs", type=str, default="120,160,200", help="where to decay lr, can be a list")
+    parser.add_argument("--lr_decay_rate", type=float, default=0.0, help="decay rate for learning rate (Adagrad's lr_decay)")
     parser.add_argument("--beta1", type=float, default=0.9, help="beta1 for adam")
     parser.add_argument("--beta2", type=float, default=0.999, help="beta2 for Adam")
     parser.add_argument("--weight-decay", type=float, default=1e-5, help="weight decay")
+    parser.add_argument("--momentum", type=float, default=0.9, help="momentum (SGD)")
     parser.add_argument("--clip-norm", type=float, default=1.0, help="clip norm")
     parser.add_argument("--resume", default="", type=str, metavar="PATH", help="path to latest checkpoint")
     parser.add_argument("--exp", type=str, default="")
@@ -101,7 +104,9 @@ def parse_option(argv=None):
     parser.add_argument("--fold-idx", type=int, default=0, help="fold of the 10-fold stratified split")
     parser.add_argument("--cv", action="store_true", help="run all 10 folds and print mean / std of the micro-F1")
     # fmt: on
-    return parser.parse_args(argv)
+    opt = parser.parse_args(argv)
+    opt.lr_decay_epochs = [int(it) for it in opt.lr_decay_epochs.split(",")]      # train.py:125-128
+    return opt
 
 
 def option_update(opt):
@@ -271,6 +276,20 @@ def test_finetune(epoch, valid_loader, model, output_layer, criterion, sw, opt):
     return epoch_loss_meter.avg, epoch_f1_meter.avg
 
 
+def make_optimizer(args, params):
+    """The encoder optimiser --optimizer names (train.py:659-681).  --lr_decay_epochs is parsed but, as in the
+    reference, unused: the per-step warm-up LR overwrites what adjust_learning_rate would set."""
+    if args.optimizer == "sgd":
+        return torch.optim.SGD(params, lr=args.learning_rate, momentum=args.momentum, weight_decay=args.weight_decay)
+    if args.optimizer == "adam":
+        return torch.optim.Adam(params, lr=args.learning_rate, betas=(args.beta1, args.beta2),
+                                weight_decay=args.weight_decay)
+    if args.optimizer == "adagrad":
+        return torch.optim.Adagrad(params, lr=args.learning_rate, lr_decay=args.lr_decay_rate,
+                                   weight_decay=args.weight_decay)
+    raise NotImplementedError(args.optimizer)
+
+
 def _make_encoder(args):
     return GraphEncoder(positional_embedding_size=args.positional_embedding_size, max_node_freq=args.max_node_freq,
                         max_edge_freq=args.max_edge_freq, max_degree=args.max_degree,
@@ -284,8 +303,8 @@ def _make_encoder(args):
 
 def main_finetune(args, dataset=None):
     """The --finetune branch of the reference's main (train.py:483-545,600-660,716-792): hyper-parameters come
-    from the pretraining checkpoint, 10-fold stratified split, BatchNorm running statistics reset, two Adam
-    optimisers, validation after the last epoch.  Returns the validation micro-F1."""
+    from the pretraining checkpoint, 10-fold stratified split, BatchNorm running statistics reset, the
+    --optimizer for the encoder and Adam for the output layer, validation after the last epoch.  Returns the validation micro-F1."""
     from sklearn.model_selection import StratifiedKFold
 
     from gcc_b200.datasets.labeled import (GRAPH_CLASSIFICATION_DSETS, GraphClassificationDatasetLabeled,
@@ -337,8 +356,7 @@ def main_finetune(args, dataset=None):
             m.reset_running_stats()
 
     model.apply(clear_bn)
-    optimizer = torch.optim.Adam(model.parameters(), lr=args.learning_rate, betas=(args.beta1, args.beta2),
-                                 weight_decay=args.weight_decay)
+    optimizer = make_optimizer(args, model.parameters())
     sw = None
     try:
         from torch.utils.tensorboard import SummaryWriter
@@ -402,7 +420,8 @@ def main(args):
     engine = PretrainEngine(train_dataset, model, model_ema, contrast, moco=args.moco,
                             learning_rate=args.learning_rate, betas=(args.beta1, args.beta2),
                             weight_decay=args.weight_decay, clip_norm=args.clip_norm, alpha=args.alpha,
-                            nce_t=args.nce_t, rank=rank, world_size=world)
+                            nce_t=args.nce_t, rank=rank, world_size=world, optimizer=args.optimizer,
+                            momentum=args.momentum, lr_decay=args.lr_decay_rate)
     sw = None
     if rank == 0:
         try:
