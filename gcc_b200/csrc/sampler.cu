@@ -19,7 +19,7 @@
 // count is known (rows with more than 128 induced neighbours are the exception: counted first, recorded on a
 // second look).  A one-hash membership filter of the frontier rejects most scanned neighbours with one shared-
 // memory load.  Hub rows (degree > 16 n) are not streamed: the ego-net's vertices are looked up in the hub's
-// sorted list, by the whole CTA at once.
+// sorted list, by the whole CTA at once; a vertex listed c times (parallel edges) is emitted c times.
 #include "common.cuh"
 
 namespace gccb {
@@ -56,14 +56,25 @@ __device__ __forceinline__ int local_id(const int* keys, int n, int seed, int u)
 // bit of the membership filter for parent id u (Knuth's multiplicative hash, top 16 bits)
 __device__ __forceinline__ unsigned bloom_bit(int u) { return ((unsigned)u * 2654435761u) >> 16; }
 
-// neighbour lists are ascending (gccb_graph_t contract): membership of u in adj(v) by bisection
-__device__ __forceinline__ bool adj_find(const int32_t* __restrict__ indices, int64_t beg, int64_t end, int u) {
+// neighbour lists are non-decreasing (gccb_graph_t contract), a value repeated c times being c parallel edges:
+// multiplicity of u in adj(v) by a lower bound, then, on a hit only, an upper bound.  A simple graph's hit costs
+// one more load, of the entry next to it.
+__device__ __forceinline__ int adj_count(const int32_t* __restrict__ indices, int64_t beg, int64_t end, int u) {
   const int64_t stop = end;
   while (beg < end) {
     int64_t mid = (beg + end) >> 1;
     if (indices[mid] < u) beg = mid + 1; else end = mid;
   }
-  return beg < stop && indices[beg] == u;
+  if (beg >= stop || indices[beg] != u) return 0;
+  // first entry > u, as a 32-bit offset from the first == u (64-bit bounds cost the fill kernel 8 registers)
+  const int32_t* run = indices + beg;
+  int lo = 1, hi = (int)min(stop - beg, (int64_t)0x7fffffff);
+  if (lo == hi || run[lo] != u) return 1;
+  while (lo < hi) {
+    int mid = (lo + hi) >> 1;
+    if (run[mid] <= u) lo = mid + 1; else hi = mid;
+  }
+  return lo;
 }
 // A hub row (parent degree >> ego-net size) is not streamed: each ego-net vertex is looked up in the
 // hub's sorted neighbour list instead (n log deg probes instead of deg reads).
@@ -80,7 +91,9 @@ __device__ __forceinline__ bool adj_find(const int32_t* __restrict__ indices, in
 #define GCCB_BLOOM 1           // A/B switches (profiles/build_variant.py)
 #endif
 #define GCCB_BLOOM_WORDS 2048   // 65,536 bits: 0.6 % false positives at n = 400, 7 % at n = 5,000
+#ifndef GCCB_HUB_LIST
 #define GCCB_HUB_LIST 1024     // hub rows per ego-net handled CTA-wide (further ones fall back to one warp each)
+#endif
 #define GCCB_HIT_STAGE 128     // hits of one row parked in shared memory before their pool slot is known
 
 // Pass 1: walk + sort/unique + induced-degree count.  grid = 2B, block = GCCB_ST.
@@ -240,17 +253,18 @@ rwr_walk_unique_kernel(const int64_t* __restrict__ indptr, const int32_t* __rest
     const int i = hub_rows[h];
     const int64_t v = keys[i];
     const int64_t beg = indptr[v], end = indptr[v + 1];
-    int cnt = 0, my_j = -1, my_ex = 0;
-    for (int t0 = 0; t0 < n; t0 += GCCB_ST) {            // count (ascending parent id, the seed spliced in at rank sr)
+    // count (ascending parent id, the seed spliced in at rank sr); a key met c times takes c consecutive slots
+    int cnt = 0, my_j = 0, my_c = 0, my_ex = 0;
+    for (int t0 = 0; t0 < n; t0 += GCCB_ST) {
       const int t = t0 + tid;
-      int j = -1;
+      int j = 0, c = 0;
       if (t < n) {
-        const int loc = t < sr ? t + 1 : (t == sr ? 0 : t);
-        if (adj_find(indices, beg, end, keys[loc])) j = loc;
+        j = t < sr ? t + 1 : (t == sr ? 0 : t);
+        c = adj_count(indices, beg, end, keys[j]);
       }
       int tot;
-      const int ex = block_scan_excl(j >= 0 ? 1 : 0, scan_scratch, &tot);
-      if (t0 == 0) { my_j = j; my_ex = ex; }
+      const int ex = block_scan_excl(c, scan_scratch, &tot);
+      if (t0 == 0) { my_j = j; my_c = c; my_ex = ex; }
       cnt += tot;
     }
     if (tid == 0) {
@@ -261,19 +275,19 @@ rwr_walk_unique_kernel(const int64_t* __restrict__ indptr, const int32_t* __rest
     const int pos = s_pos;
     if (pos >= 0) {
       if (n <= GCCB_ST) {
-        if (my_j >= 0) pool[pos + my_ex] = my_j;
+        for (int k = 0; k < my_c; ++k) pool[pos + my_ex + k] = my_j;
       } else {
         int w = 0;
         for (int t0 = 0; t0 < n; t0 += GCCB_ST) {
           const int t = t0 + tid;
-          int j = -1;
+          int j = 0, c = 0;
           if (t < n) {
-            const int loc = t < sr ? t + 1 : (t == sr ? 0 : t);
-            if (adj_find(indices, beg, end, keys[loc])) j = loc;
+            j = t < sr ? t + 1 : (t == sr ? 0 : t);
+            c = adj_count(indices, beg, end, keys[j]);
           }
           int tot;
-          const int ex = block_scan_excl(j >= 0 ? 1 : 0, scan_scratch, &tot);
-          if (j >= 0) pool[pos + w + ex] = j;
+          const int ex = block_scan_excl(c, scan_scratch, &tot);
+          for (int k = 0; k < c; ++k) pool[pos + w + ex + k] = j;
           w += tot;
         }
       }
@@ -309,15 +323,21 @@ rwr_walk_unique_kernel(const int64_t* __restrict__ indptr, const int32_t* __rest
       w = 0;
       if (reverse) {
         // hub row (beyond the CTA-wide list): probe adj(v) for every ego-net vertex in ascending parent id (= the
-        // order a scan of adj(v) would meet them): keys[1..n) is ascending, the seed (local id 0) is spliced in at rank sr
+        // order a scan of adj(v) would meet them): keys[1..n) is ascending, the seed (local id 0) is spliced in at rank sr.
+        // A key met c times (parallel edges) takes c consecutive slots: a warp prefix sum of the counts.
         for (int t0 = 0; t0 < n; t0 += 32) {
           const int t = t0 + lane;
-          int j = -1;
+          int j = 0, c = 0;
           if (t < n) {
-            const int loc = t < sr ? t + 1 : (t == sr ? 0 : t);
-            if (adj_find(indices, beg, end, keys[loc])) j = loc;
+            j = t < sr ? t + 1 : (t == sr ? 0 : t);
+            c = adj_count(indices, beg, end, keys[j]);
           }
-          emit(j);
+          const int incl = warp_scan_incl(c, lane);
+          for (int q = w + incl - c; q < w + incl; ++q) {
+            if (round == 1) pool[pos + q] = j;
+            else if (q < GCCB_HIT_STAGE) wstage[q] = j;
+          }
+          w += __shfl_sync(0xffffffffu, incl, 31);
         }
       } else {
         // four independent 128-byte loads in flight per warp before the first search: the scan of a cold
@@ -484,14 +504,14 @@ induce_fill_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict
       const int sr = lo - 1;                             // number of non-seed keys below the seed
       for (int t0 = 0; t0 < n; t0 += 32) {
         const int t = t0 + lane;
-        int j = -1;
+        int j = 0, c = 0;
         if (t < n) {
-          const int loc = t < sr ? t + 1 : (t == sr ? 0 : t);
-          if (adj_find(indices, beg, end, keys[loc])) j = loc;
+          j = t < sr ? t + 1 : (t == sr ? 0 : t);
+          c = adj_count(indices, beg, end, keys[j]);
         }
-        unsigned hit = __ballot_sync(0xffffffffu, j >= 0);
-        if (j >= 0) v_indices[wpos + __popc(hit & ((1u << lane) - 1u))] = noff + j;
-        wpos += __popc(hit);
+        const int incl = warp_scan_incl(c, lane);      // parallel edges: c consecutive slots
+        for (int q = wpos + incl - c; q < wpos + incl; ++q) v_indices[q] = noff + j;
+        wpos += __shfl_sync(0xffffffffu, incl, 31);
       }
       continue;
     }

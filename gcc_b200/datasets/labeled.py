@@ -106,10 +106,11 @@ def graph_from_edge_index(edge_index, num_nodes=None):
     return synthetic.CSRGraph(indptr, d.astype(np.int32), n, "edge_index")
 
 
-def read_tu_dataset(root, name):
+def read_tu_dataset(root, name, multigraph=False):
     """The public TU layout: <name>_A.txt ("u, v" 1-based, both directions listed), <name>_graph_indicator.txt
     (graph id of node i, 1-based), <name>_graph_labels.txt.  Returns (list[CSRGraph], int64 labels numbered from 0
-    in order of sorted distinct values, like dgl.data.TUDataset)."""
+    in order of sorted distinct values, like dgl.data.TUDataset).  multigraph=True keeps every listed entry once,
+    repeated pairs and self loops included, as dgl.data.TUDataset's graphs do; the default makes simple graphs."""
     base = os.path.join(root, name, name)
     ind = np.loadtxt(base + "_graph_indicator.txt", dtype=np.int64).reshape(-1) - 1
     a = np.loadtxt(base + "_A.txt", dtype=np.int64, delimiter=",").reshape(-1, 2) - 1
@@ -128,8 +129,18 @@ def read_tu_dataset(root, name):
     bounds = np.searchsorted(gid, np.arange(n_graphs + 1))
     for g in range(n_graphs):
         e = a[bounds[g]:bounds[g + 1]] - first[g]
-        graphs.append(_simple_csr(e[:, 0], e[:, 1], int(sizes[g]), "%s_%d" % (name, g)))
+        make = _listed_csr if multigraph else _simple_csr
+        graphs.append(make(e[:, 0], e[:, 1], int(sizes[g]), "%s_%d" % (name, g)))
     return graphs, labels
+
+
+def _listed_csr(src, dst, n, name):
+    """CSR of the directed entries src -> dst exactly as listed (rows non-decreasing), isolated vertices kept."""
+    src, dst = np.asarray(src, dtype=np.int64), np.asarray(dst, dtype=np.int64)
+    order = np.lexsort((dst, src))
+    indptr = np.zeros(n + 1, dtype=np.int64)
+    np.cumsum(np.bincount(src, minlength=n), out=indptr[1:])
+    return synthetic.CSRGraph(indptr, dst[order].astype(np.int32), n, name)
 
 
 def _simple_csr(src, dst, n, name):

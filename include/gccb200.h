@@ -51,10 +51,15 @@ const char* gccb_last_error(void);
 /* number of kernels this library has enqueued so far in this process (host counter) */
 unsigned long long gccb_launch_count(void);
 
-/* ---- parent graph + sampler constants (host struct, device pointers inside) -------- */
+/* ---- parent graph + sampler constants (host struct, device pointers inside) --------
+ * Row v of the CSR lists the heads of v's out-edges, NON-DECREASING: a neighbour repeated c
+ * times is c parallel edges (a DGL multigraph keeps them).  A walk step picks each entry with
+ * equal probability, so u with probability c/deg(v); the induced ego-net keeps all c copies,
+ * in the order a scan of the row meets them, and sub_deg counts them.  Self loops are allowed
+ * and kept.  Every vertex needs an out-edge.                                               */
 typedef struct {
   const int64_t* indptr;       /* [n_nodes+1] CSR row offsets                                */
-  const int32_t* indices;      /* [nnz] neighbour ids, ascending per row                     */
+  const int32_t* indices;      /* [nnz] neighbour ids, non-decreasing per row (see above)    */
   int64_t n_nodes;
   const int32_t* budget_table; /* [budget_table_len] max_nodes_per_seed by seed degree:
                                   graph_dataset.py:113-124, built on the host               */
