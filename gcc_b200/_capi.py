@@ -28,6 +28,10 @@ class Batch(C.Structure):
                 ("counters", p), ("flags", p)]
 
 
+class GraphSet(C.Structure):
+    _fields_ = [("indptr", p), ("indices", p), ("node_off", p), ("edge_off", p), ("n_graphs", C.c_int64)]
+
+
 class GinCfg(C.Structure):
     _fields_ = [("num_layers", C.c_int32), ("hidden", C.c_int32), ("pos_dim", C.c_int32),
                 ("deg_dim", C.c_int32), ("max_degree", C.c_int32), ("norm", C.c_int32),
@@ -57,6 +61,7 @@ _PROTOS = {
     "gccb_draw_seeds": (C.c_int, [p, C.c_int64, C.c_uint64, C.c_int64, C.c_int32, p, p, p]),
     "gccb_sample_batch_workspace": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32]),
     "gccb_sample_batch": (C.c_int, [C.POINTER(Graph), p, p, C.POINTER(Batch), p, C.c_size_t, p]),
+    "gccb_gather_graphs": (C.c_int, [C.POINTER(GraphSet), p, C.POINTER(Batch), p]),
     "gccb_posenc_workspace": (C.c_size_t, [C.c_int32, C.c_int32]),
     "gccb_posenc": (C.c_int, [C.POINTER(Batch), C.c_int32, C.c_int32, p, p, p, C.c_size_t, p]),
     "gccb_gin_param_layout": (C.c_int, [C.POINTER(GinCfg), C.POINTER(GinLayout)]),

@@ -15,6 +15,7 @@ positional features and batching all run as CUDA kernels over a CSR kept in HBM:
 Randomness is the counter-based "RWR-Philox v1" stream (DESIGN.md), so a batch is a
 pure function of (run seed, sample ids) -- independent of worker count or world size.
 """
+import copy
 import ctypes as C
 import math
 import operator
@@ -101,12 +102,15 @@ class DeviceGraph:
 
 
 class BatchBuffers:
-    """Caller-owned device memory behind one gccb_batch_t (both views of B pairs)."""
+    """Caller-owned device memory behind one gccb_batch_t (both views of B pairs).  max_budget sizes the
+    sampler's workspace; None for buffers that only whole-graph batches fill (gccb_gather_graphs needs none)."""
 
     def __init__(self, B, node_cap, edge_cap, pos_dim, max_budget, device):
         lib = _lib.get()
         i32 = dict(dtype=torch.int32, device=device)
         self.B, self.node_cap, self.edge_cap, self.pos_dim = B, node_cap, edge_cap, pos_dim
+        self.max_budget = max_budget
+        self._narrowed = {}
         self.node_off = torch.zeros(2, B + 1, **i32)
         self.edge_off = torch.zeros(2, B + 1, **i32)
         self.indptr = torch.zeros(2, node_cap + 1, **i32)
@@ -120,15 +124,38 @@ class BatchBuffers:
         self.eigvals = torch.zeros(2 * B, pos_dim, dtype=torch.float32, device=device)
         self.seeds = torch.zeros(B, dtype=torch.int64, device=device)
         self.sample_ids = torch.zeros(B, dtype=torch.int64, device=device)
-        self.ws_sample = torch.zeros(max(lib.gccb_sample_batch_workspace(B, max_budget, edge_cap), 8),
-                                     dtype=torch.uint8, device=device)
+        ws = lib.gccb_sample_batch_workspace(B, max_budget, edge_cap) if max_budget is not None else 0
+        self.ws_sample = torch.zeros(max(ws, 8), dtype=torch.uint8, device=device)
         self.ws_posenc = torch.zeros(max(lib.gccb_posenc_workspace(B, node_cap), 8),
                                      dtype=torch.uint8, device=device)
-        self.c = _capi.Batch(B, node_cap, edge_cap, 0, self.node_off.data_ptr(),
-                             self.edge_off.data_ptr(), self.indptr.data_ptr(),
-                             self.indices.data_ptr(), self.sub_deg.data_ptr(),
-                             self.graph_id.data_ptr(), self.orig_id.data_ptr(),
-                             self.counters.data_ptr(), self.flags.data_ptr())
+        self.c = self._batch_struct()
+
+    def _batch_struct(self):
+        return _capi.Batch(self.B, self.node_cap, self.edge_cap, 0, self.node_off.data_ptr(),
+                           self.edge_off.data_ptr(), self.indptr.data_ptr(),
+                           self.indices.data_ptr(), self.sub_deg.data_ptr(),
+                           self.graph_id.data_ptr(), self.orig_id.data_ptr(),
+                           self.counters.data_ptr(), self.flags.data_ptr())
+
+    def narrow(self, b):
+        """The same memory as a batch of b <= B pairs (the short last batch of an epoch): node_off / edge_off
+        laid out [2][b+1] and counters [2b][4] at the front of the full arrays, every per-node array, the flag
+        word and the workspaces shared.  Cached per b; narrow(B) is these buffers."""
+        if b == self.B:
+            return self
+        if not 0 < b < self.B:
+            raise ValueError("a batch of %d pairs does not fit buffers of %d" % (b, self.B))
+        if b not in self._narrowed:
+            s = copy.copy(self)
+            s.B, s._narrowed = b, {}
+            s.node_off = self.node_off.view(-1)[:2 * (b + 1)].view(2, b + 1)
+            s.edge_off = self.edge_off.view(-1)[:2 * (b + 1)].view(2, b + 1)
+            s.counters = self.counters[:2 * b]
+            s.eigvals = self.eigvals[:2 * b]
+            s.seeds, s.sample_ids = self.seeds[:b], self.sample_ids[:b]
+            s.c = s._batch_struct()
+            self._narrowed[b] = s
+        return self._narrowed[b]
 
     def eig_debug(self):
         """(iterations, worst residual) per ego-net of the last gccb_posenc on these buffers, read
@@ -254,13 +281,37 @@ class LoadBalanceGraphDataset(torch.utils.data.IterableDataset):
             yield BatchedSubgraphs(buf, 0), BatchedSubgraphs(buf, 1)
 
 
-class NodeClassificationDataset:
+class _EpochOrder:
+    """Pretraining on a downstream dataset (train.py:547-586): the reference's map-style DataLoader with
+    shuffle=False, drop_last=False.  An epoch is items 0..total-1 in order, in batches of B; the last one holds
+    total mod B items when that is not 0.  PretrainEngine numbers its batches j = 0, 1, ... and asks for batch j
+    with first_sample = j * B (parallel.first_sample_id on one GPU); j counts on across epochs.  The reference
+    trains these datasets on one GPU only, so the engine refuses world_size > 1 for them."""
+
+    epoch_ordered = True
+
+    def steps_per_epoch(self):
+        return -(-self.total // self.batch_size)
+
+    def _locate(self, first_sample):
+        """(epoch, first item, item count) of the engine's batch that starts at first_sample."""
+        B = self.batch_size
+        if first_sample is None:
+            first_sample = self.next_batch * B
+            self.next_batch += 1
+        epoch, idx = divmod(int(first_sample) // B, self.steps_per_epoch())
+        a = idx * B
+        return epoch, a, min(B, self.total - a)
+
+
+class NodeClassificationDataset(_EpochOrder):
     """generate.py's dataset (graph_dataset.py:279-309 on top of GraphDataset :218-275): item idx is
     NODE idx of one graph, seeds are taken in order (no sampling), both views walk from the seed
     (step_dist [1,0,0]) with budget max(rw_hops, int(deg*e/(e-1)/restart + 0.5)) -- plain degree,
     unlike the pretraining loader.  `dataset` is a CSRGraph or an .npz path (the reference's
     downloaded datasets need the network / DGL).  Iterating yields batched (graph_q, graph_k, count)
-    with `count` valid pairs (the last batch is padded with the last node)."""
+    with `count` valid pairs (the last batch is padded with the last node).  sample_batch() is the
+    pretraining interface (see _EpochOrder)."""
 
     def __init__(self, dataset, rw_hops=64, subgraph_size=64, restart_prob=0.8,
                  positional_embedding_size=32, step_dist=[1.0, 0.0, 0.0], device="cuda", seed=0,
@@ -281,6 +332,7 @@ class NodeClassificationDataset:
         self.edge_cap = int(edge_cap or self.node_cap * 16)
         self.buffers = BatchBuffers(B, self.node_cap, self.edge_cap, positional_embedding_size, mb, self.device)
         self._sampler = LoadBalanceGraphDataset.sample_batch
+        self.next_batch = 0
 
     def __len__(self):
         return self.length
@@ -293,5 +345,98 @@ class NodeClassificationDataset:
             buf = self._sampler(self, first_sample=start, seeds=seeds)
             buf.check_flags()
             yield BatchedSubgraphs(buf, 0), BatchedSubgraphs(buf, 1), count
+
+    def sample_batch(self, first_sample=None, seeds=None, buffers=None, posenc=True):
+        """Batch number first_sample // B of the epoch order, on the device with no host sync: seeds are the
+        epoch's items a .. a+b-1, and Philox sample id epoch * total + item gives every item fresh walk randomness
+        in every epoch (sample ids are never reused).  Returns the buffers narrowed to the b pairs."""
+        if seeds is not None:
+            raise ValueError("a node dataset trains on its nodes in order: the seeds are not the caller's")
+        epoch, a, b = self._locate(first_sample)
+        buf = (buffers or self.buffers).narrow(b)
+        lib = _lib.get()
+        torch.arange(a, a + b, device=self.device, out=buf.seeds)
+        base = epoch * self.total
+        torch.arange(base + a, base + a + b, device=self.device, out=buf.sample_ids)
+        _lib.check(lib.gccb_sample_batch(C.byref(self.graph.c), _lib.dptr(buf.seeds), _lib.dptr(buf.sample_ids),
+                                         C.byref(buf.c), _lib.dptr(buf.ws_sample), buf.ws_sample.numel(),
+                                         _lib.stream_ptr()), "gccb_sample_batch")
+        if posenc:
+            self.posenc(buf)
+        return buf
+
+    posenc = LoadBalanceGraphDataset.posenc
+
+
+def seed_first_union(graphs):
+    """Every graph relabelled seed first -- its first maximum out-degree vertex (graph_dataset.py:361) moved to
+    row 0 by labeled.seed_first -- and the set as one union CSR (the gccb_graph_set_t layout).  Returns (seeds,
+    items = [(indptr, indices)] per relabelled graph, indptr, indices as union ids, node_off, edge_off), int64."""
+    from .labeled import seed_first
+    seeds = np.array([int(np.argmax(np.diff(g.indptr))) for g in graphs], dtype=np.int64)
+    items = [seed_first(g.indptr, g.indices, s)[:2] for g, s in zip(graphs, seeds)]
+    node_off = np.concatenate([[0], np.cumsum([len(ip) - 1 for ip, _ in items])]).astype(np.int64)
+    edge_off = np.concatenate([[0], np.cumsum([len(ix) for _, ix in items])]).astype(np.int64)
+    indptr = np.concatenate([ip[:-1] + e for (ip, _), e in zip(items, edge_off)] + [edge_off[-1:]])
+    indices = np.concatenate([np.asarray(ix, dtype=np.int64) + a for (_, ix), a in zip(items, node_off)])
+    return seeds, items, indptr.astype(np.int64), indices, node_off, edge_off
+
+
+class GraphClassificationDataset(_EpochOrder):
+    """graph_dataset.py:311-340 (entire_graph=True) for pretraining: item idx is GRAPH idx, and q and k are
+    both the whole graph with its seed on the first maximum out-degree vertex.  The reference also walks an
+    RWR trace per view and then discards it; nothing is walked here.  Each graph is relabelled seed first
+    once, here (labeled.seed_first), and the set lives on the device as one union CSR; a batch is
+    gccb_gather_graphs of the epoch's next graph ids.  Positional features come from a deterministic
+    eigensolver, so the two views' features are identical (the reference starts ARPACK from a random vector
+    per view).  `dataset` is a name of downstream.GRAPH_DSETS (TU files under ./data), a list of CSRGraphs or
+    a (graphs, labels) pair; the graphs keep their listed multi-edges (downstream.graph_dataset_graphs)."""
+
+    def __init__(self, dataset, rw_hops=64, subgraph_size=64, restart_prob=0.8, positional_embedding_size=32,
+                 step_dist=[1.0, 0.0, 0.0], device="cuda", seed=0, batch_size=32):
+        from . import downstream
+        assert positional_embedding_size > 1
+        self.rw_hops, self.subgraph_size, self.restart_prob = rw_hops, subgraph_size, restart_prob
+        self.positional_embedding_size, self.step_dist = positional_embedding_size, step_dist
+        self.entire_graph = True
+        if isinstance(dataset, str):
+            graphs, _ = downstream.graph_dataset_graphs(dataset)
+        elif isinstance(dataset, tuple) and len(dataset) == 2:
+            graphs = list(dataset[0])
+        else:
+            graphs = list(dataset)
+        self.length = self.total = len(graphs)
+        self.seeds, self.items, indptr, indices, node_off, edge_off = seed_first_union(graphs)
+        sizes, nnz = np.diff(node_off), np.diff(edge_off)
+        self.device = torch.device(device)
+        _lib.require_device()
+        to = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a)).to(device=self.device, dtype=dt)
+        self.indptr, self.indices = to(indptr, torch.int64), to(indices, torch.int32)
+        self.node_off, self.edge_off = to(node_off, torch.int64), to(edge_off, torch.int64)
+        self.c = _capi.GraphSet(self.indptr.data_ptr(), self.indices.data_ptr(), self.node_off.data_ptr(),
+                                self.edge_off.data_ptr(), self.total)
+        self.batch_size = B = int(min(batch_size, self.total))
+        # capacity of the B largest graphs (labeled.GraphClassificationDatasetLabeled._new_buffers)
+        self.node_cap = int(np.sort(sizes)[::-1][:B].sum()) + 8
+        self.edge_cap = int(np.sort(nnz)[::-1][:B].sum()) + 8
+        self.buffers = BatchBuffers(B, self.node_cap, self.edge_cap, positional_embedding_size, None, self.device)
+        self.next_batch = 0
+
+    def __len__(self):
+        return self.length
+
+    def sample_batch(self, first_sample=None, seeds=None, buffers=None, posenc=True):
+        """Batch number first_sample // B of the epoch order: graphs a .. a+b-1 in both views, on the device with
+        no host sync.  Returns the buffers narrowed to the b pairs."""
+        if seeds is not None:
+            raise ValueError("a graph dataset trains on its graphs in order: the seeds are not the caller's")
+        _, a, b = self._locate(first_sample)
+        buf = (buffers or self.buffers).narrow(b)
+        torch.arange(a, a + b, device=self.device, out=buf.seeds)
+        _lib.check(_lib.get().gccb_gather_graphs(C.byref(self.c), _lib.dptr(buf.seeds), C.byref(buf.c),
+                                                 _lib.stream_ptr()), "gccb_gather_graphs")
+        if posenc:
+            self.posenc(buf)
+        return buf
 
     posenc = LoadBalanceGraphDataset.posenc

@@ -34,6 +34,9 @@ class PretrainEngine:
         eps 1e-10), as train.py:659-678 builds them over model.parameters()."""
         if optimizer not in ("adam", "sgd", "adagrad"):
             raise ValueError("optimizer must be adam, sgd or adagrad, not %r" % (optimizer,))
+        if world_size > 1 and getattr(dataset, "epoch_ordered", False):
+            raise ValueError("%s: the reference trains node and graph datasets on one GPU; use world_size 1"
+                             % type(dataset).__name__)
         _lib.require_device()
         self.lib = _lib.get()
         self.ds, self.model, self.model_ema, self.contrast = dataset, model, model_ema, contrast
@@ -71,6 +74,7 @@ class PretrainEngine:
         self.stats = self.xch.stats_send if self.xch else torch.zeros(4, **f32)
         self.stats_acc = torch.zeros(4, dtype=torch.float64, device=dev)   # per-step sums since the last read_stats()
         self.steps_acc = 0
+        self.pairs_acc = 0                             # pairs trained since the last read_stats()
         self.norm_ws = torch.zeros(1, dtype=torch.float64, device=dev)
         self.any_skip = torch.zeros(1, dtype=torch.int32, device=dev)
         self.feat_q = torch.zeros(B, H, **f32)
@@ -111,7 +115,8 @@ class PretrainEngine:
             S = self.prefetch
             self.depth = S + 1
             self.bufs = [ds.buffers] + [BatchBuffers(B, ds.node_cap, ds.edge_cap, ds.buffers.pos_dim,
-                                                     ds.graph.max_budget, dev) for _ in range(S)]
+                                                     ds.buffers.max_budget, dev) for _ in range(S)]
+            self.slot_bufs = list(self.bufs)           # what each slot holds: its buffers, or them narrowed
             self.data_streams = [self._new_stream(1, 0) for _ in range(S)]
             self.ready = [torch.cuda.Event() for _ in range(self.depth)]
             self.consumed = [torch.cuda.Event() for _ in range(self.depth)]
@@ -166,7 +171,8 @@ class PretrainEngine:
                 t = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
                 t[0].record()
             first = first_sample_id(j, self.world, self.rank, self.B)
-            self.ds.sample_batch(first_sample=first, seeds=seeds, buffers=buf, posenc=False)
+            buf = self.ds.sample_batch(first_sample=first, seeds=seeds, buffers=buf, posenc=False)
+            self.slot_bufs[slot] = buf                 # an epoch's short last batch: fewer pairs, same memory
             if t:
                 t[1].record()
             self.ds.posenc(buf)
@@ -210,7 +216,7 @@ class PretrainEngine:
                 seeds = None        # warm-up: only the first batch of a multi-batch fill takes the caller's seeds,
                                     # the others are drawn on the device (no duplicated batches)
             slot = self.global_step % self.depth
-            buf = self.bufs[slot]
+            buf = self.slot_bufs[slot]
             torch.cuda.current_stream(self.dev).wait_event(self.ready[slot])
         else:
             first = first_sample_id(self.global_step, self.world, self.rank, B)
@@ -222,6 +228,9 @@ class PretrainEngine:
         if self.count_acc is not None:
             self.count_acc += buf.counters.double().sum(0)
         gq, gk = BatchedSubgraphs(buf, 0), BatchedSubgraphs(buf, 1)
+        # pairs in this batch: B, or fewer in the last batch of an epoch of a node / graph dataset.  The feature and
+        # gradient buffers are [B][H]; the kernels use their first b rows
+        b = buf.B
         step = self.global_step
         if self.moco:
             # the key encoder (model_ema, its own weights and running statistics) is independent of
@@ -237,7 +246,7 @@ class PretrainEngine:
         if self.moco:
             cur.wait_stream(self.aux_stream)
             _lib.check(lib.gccb_infonce_fused(_lib.dptr(self.feat_q), _lib.dptr(self.feat_k),
-                                              _lib.dptr(self.contrast.memory), B, H, self.K, self.T,
+                                              _lib.dptr(self.contrast.memory), b, H, self.K, self.T,
                                               _lib.dptr(self.stats), _lib.dptr(self.dq),
                                               _lib.dptr(self.nce_ws), self.nce_ws.numel(), st),
                        "gccb_infonce_fused")
@@ -245,7 +254,7 @@ class PretrainEngine:
         else:
             _, _, saved_k = model._run_forward(gk, True, drop_step=step, drop_base=L, acts=self.acts_k,
                                                feat=self.feat_k, pooled=self.pooled, bn_train=True)
-            _lib.check(lib.gccb_e2e_nce(_lib.dptr(self.feat_q), _lib.dptr(self.feat_k), B, H, self.T,
+            _lib.check(lib.gccb_e2e_nce(_lib.dptr(self.feat_q), _lib.dptr(self.feat_k), b, H, self.T,
                                         _lib.dptr(self.stats), _lib.dptr(self.dq), _lib.dptr(self.dk),
                                         _lib.dptr(self.nce_ws), self.nce_ws.numel(), st), "gccb_e2e_nce")
             model._run_backward(gq, saved_q, self.dq, grads_flat=self.grads, ws=self.bwd_ws)
@@ -283,15 +292,20 @@ class PretrainEngine:
         if self.moco:
             # all ranks' keys in rank order with one launch -> identical queues on every rank
             src = self.xch.gathered if self.world > 1 else self.feat_k
-            _lib.check(lib.gccb_moco_enqueue(_lib.dptr(self.contrast.memory), _lib.dptr(src), B, H, self.K,
+            _lib.check(lib.gccb_moco_enqueue(_lib.dptr(self.contrast.memory), _lib.dptr(src), b, H, self.K,
                                              _lib.dptr(self.index_dev), self.world,
                                              self.payload if self.world > 1 else 0, skip_word, skip_mask, st),
                        "gccb_moco_enqueue")
-            self.contrast.index = (self.contrast.index + B * self.world) % self.K
+            self.contrast.index = (self.contrast.index + b * self.world) % self.K
         # the reference updates its meters from .item() reads every step (train.py:420-428); here the
         # per-step scalars are summed on the device and read on demand
-        self.stats_acc.add_(self.stats)
+        if b == B:
+            self.stats_acc.add_(self.stats)
+        else:                                          # loss and prob weighted by pairs, as the reference's meters
+            self.stats_acc[:2].add_(self.stats[:2], alpha=b / B)
+            self.stats_acc[2:].add_(self.stats[2:])
         self.steps_acc += 1
+        self.pairs_acc += b
         if self.timing_main is not None:
             tm[1].record()
             self.timing_main.append(tm)
@@ -307,20 +321,24 @@ class PretrainEngine:
                 cur.wait_stream(ds_)
 
     def read_stats(self):
-        """Host sync: loss, prob (mean positive logit), pre-clip grad norm, batch sizes, flags."""
+        """Host sync: loss, prob (mean positive logit), pre-clip grad norm, sizes of the batch the last step
+        trained on, flags.  window_loss / window_prob average over the window's pairs (window_pairs), the
+        grad norm over its steps."""
         buf = self.cur_buf
         torch.cuda.synchronize(self.dev)
         for b_ in (self.bufs if self.prefetch else [buf]):     # every buffer of the run-ahead ring, not only
             b_.check_flags()                                   # the one the last step trained on
         s = self.stats.tolist()
         acc, w = self.stats_acc.tolist(), max(self.steps_acc, 1)
+        wp = self.pairs_acc / self.B if self.pairs_acc else 1      # = w when every batch is full
         self.stats_acc.zero_()
-        window = self.steps_acc
-        self.steps_acc = 0
-        sizes = buf.node_off[:, self.B].tolist() + buf.edge_off[:, self.B].tolist()
+        window, pairs = self.steps_acc, self.pairs_acc
+        self.steps_acc = self.pairs_acc = 0
+        sizes = buf.node_off[:, buf.B].tolist() + buf.edge_off[:, buf.B].tolist()
         return dict(loss=s[0], prob=s[1], grad_norm=s[2], nodes_q=sizes[0], nodes_k=sizes[1],
-                    edges_q=sizes[2], edges_k=sizes[3], window_steps=window, window_loss=acc[0] / w,
-                    window_prob=acc[1] / w, window_grad_norm=acc[2] / w)
+                    edges_q=sizes[2], edges_k=sizes[3], batch_size=buf.B, window_steps=window,
+                    window_pairs=pairs, window_loss=acc[0] / wp, window_prob=acc[1] / wp,
+                    window_grad_norm=acc[2] / w)
 
     def optimizer_state_dict(self):
         """The flat optimiser buffers in the layout of torch.optim.{Adam,SGD,Adagrad}(model.parameters())

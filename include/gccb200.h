@@ -112,6 +112,27 @@ int gccb_sample_batch(const gccb_graph_t* graph, const int64_t* seeds,
                       const int64_t* sample_ids, const gccb_batch_t* batch, void* workspace,
                       size_t workspace_bytes, gccb_stream_t stream);
 
+/* Whole-graph batches (entire_graph=True, graph_dataset.py:311-340; dgl.batch, data_util.py:26-32).
+ * A set of graphs as one union CSR: graph i owns vertices node_off[i] .. node_off[i+1) and entries
+ * edge_off[i] .. edge_off[i+1) (= indptr[node_off[i]] ..), rows as listed (parallel edges, self loops and
+ * isolated vertices are kept), `indices` holding union vertex ids.  Each graph must already be relabelled
+ * seed first: row 0 is the seed.                                                                          */
+typedef struct {
+  const int64_t* indptr;   /* [n_nodes+1] union CSR row offsets      */
+  const int32_t* indices;  /* [nnz] union vertex ids                 */
+  const int64_t* node_off; /* [n_graphs+1] first vertex of graph i   */
+  const int64_t* edge_off; /* [n_graphs+1] first entry of graph i    */
+  int64_t n_graphs;
+} gccb_graph_set_t;
+
+/* Both views of `batch` = the graphs graph_ids[0..B) (device int64, clamped to the set), identical:
+ * node_off / edge_off, view-local indptr / indices, sub_deg = row length, graph_id, orig_id = the view-local
+ * row, counters (n, m, 0, 0).  A view that exceeds node_cap / edge_cap raises GCCB_FLAG_NODE_OVERFLOW /
+ * GCCB_FLAG_EDGE_OVERFLOW and is published empty (node_off[v][B] = edge_off[v][B] = -1), as in
+ * gccb_sample_batch.  No workspace, no host sync.                                                       */
+int gccb_gather_graphs(const gccb_graph_set_t* set, const int64_t* graph_ids, const gccb_batch_t* batch,
+                       gccb_stream_t stream);
+
 /* A5  Laplacian positional features.  Replaces
  * _add_undirected_graph_positional_embedding + eigen_decomposision
  * (data_util.py:242-281): top-k (k = min(n-2, pos_dim)) eigenvectors of

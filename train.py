@@ -34,8 +34,9 @@ import numpy as np
 import torch
 
 from gcc_b200.contrastive.memory_moco import MemoryMoCo
-from gcc_b200.datasets import synthetic
-from gcc_b200.datasets.graph_dataset import LoadBalanceGraphDataset
+from gcc_b200.datasets import downstream, synthetic
+from gcc_b200.datasets.graph_dataset import (GraphClassificationDataset, LoadBalanceGraphDataset,
+                                             NodeClassificationDataset)
 from gcc_b200.engine import PretrainEngine
 from gcc_b200.models import GraphEncoder
 from gcc_b200.utils.misc import AverageMeter, warmup_linear
@@ -66,7 +67,9 @@ def parse_option(argv=None):
     parser.add_argument("--exp", type=str, default="")
     # dataset definition
     parser.add_argument("--dataset", type=str, default="synthetic-chunglu",
-                        help="synthetic-chunglu | synthetic-er | path to .npz(indptr, indices[, graph_sizes])")
+                        help="synthetic-chunglu | synthetic-er | dgl (./data/small.bin) | a downstream node or graph "
+                             "dataset (%s; files under ./data) | path to .npz(indptr, indices[, graph_sizes]) or DGL "
+                             ".bin" % ", ".join(downstream.NODE_DSETS + downstream.GRAPH_DSETS))
     parser.add_argument("--graph-nodes", type=int, default=1000000)
     parser.add_argument("--graph-edges", type=int, default=20000000)
     # model definition
@@ -130,30 +133,52 @@ def build_graph(args, device):
         return synthetic.chung_lu_device(args.graph_nodes, args.graph_edges, 0.5, seed=0, device=device)
     if args.dataset == "synthetic-er":
         return synthetic.erdos_renyi(args.graph_nodes, args.graph_edges, seed=0)
-    return args.dataset          # path to .npz
+    if args.dataset == "dgl":
+        return "./data/small.bin"    # the reference's default pretraining corpus (train.py:547-556)
+    return args.dataset          # path to .npz or .bin
+
+
+def build_dataset(args, device):
+    """The reference's three branches (train.py:547-573): a downstream node dataset (every node of its multigraph
+    in order), a TU graph dataset (every whole graph in order), else the sampled ego-nets of
+    LoadBalanceGraphDataset over the corpus build_graph names."""
+    kw = dict(rw_hops=args.rw_hops, restart_prob=args.restart_prob,
+              positional_embedding_size=args.positional_embedding_size, batch_size=args.batch_size, seed=args.seed,
+              device=device)
+    if args.dataset in downstream.NODE_DSETS:
+        return NodeClassificationDataset(downstream.node_dataset_graph(args.dataset),
+                                         subgraph_size=args.subgraph_size, **kw)
+    if args.dataset in downstream.GRAPH_DSETS:
+        return GraphClassificationDataset(args.dataset, subgraph_size=args.subgraph_size, **kw)
+    return LoadBalanceGraphDataset(num_workers=args.num_workers, num_samples=args.num_samples,
+                                   dgl_graphs_file=build_graph(args, device), num_copies=args.num_copies, **kw)
 
 
 def train_moco(epoch, engine, sw, opt, is_main):
-    """One epoch (train.py:350-478): n_batch = dataset.total // batch_size steps."""
+    """One epoch (train.py:350-478): n_batch = dataset.total // batch_size steps.  A node or graph dataset also
+    trains its last total mod batch_size items as a short batch (the reference's DataLoader keeps it); the LR
+    schedule keeps n_batch, so that batch runs at idx = n_batch."""
     n_batch = engine.ds.total // (opt.batch_size * engine.world)
     if n_batch == 0:
         raise ValueError("dataset.total = %d is smaller than one global batch (%d x %d): nothing to train on"
                          % (engine.ds.total, opt.batch_size, engine.world))
+    n_steps = engine.ds.steps_per_epoch() if getattr(engine.ds, "epoch_ordered", False) else n_batch
     loss_meter, prob_meter, gs_meter, gnorm_meter = (AverageMeter() for _ in range(4))
     epoch_loss, batch_time = AverageMeter(), AverageMeter()
     end = time.time()
     max_nodes = max_edges = 0
-    for idx in range(n_batch):
+    for idx in range(n_steps):
         global_step = epoch * n_batch + idx
         lr = opt.learning_rate * warmup_linear(global_step / (opt.epochs * n_batch), 0.1)   # train.py:411-416
         engine.step(lr=lr)
-        if (idx + 1) % opt.print_freq == 0 or idx + 1 == n_batch:
+        if (idx + 1) % opt.print_freq == 0 or idx + 1 == n_steps:
             s = engine.read_stats()                      # the only host sync of the window
-            bsz = opt.batch_size
+            bsz = s["batch_size"]                        # of the last step: opt.batch_size but for a short batch
             w = max(s["window_steps"], 1)                # device-side sums over every step since the last read
-            loss_meter.update(s["window_loss"], bsz * w)
-            epoch_loss.update(s["window_loss"], bsz * w)
-            prob_meter.update(s["window_prob"], bsz * w)
+            pairs = s["window_pairs"]                    # the meters weight each step by its pairs, as the reference
+            loss_meter.update(s["window_loss"], pairs)
+            epoch_loss.update(s["window_loss"], pairs)
+            prob_meter.update(s["window_prob"], pairs)
             gs_meter.update((s["nodes_q"] + s["nodes_k"]) / 2.0 / bsz, 2 * bsz)
             gnorm_meter.update(s["window_grad_norm"], w)
             max_nodes, max_edges = max(max_nodes, s["nodes_q"]), max(max_edges, s["edges_q"])
@@ -162,7 +187,7 @@ def train_moco(epoch, engine, sw, opt, is_main):
             if is_main:
                 print("Train: [{0}][{1}/{2}]\tBT {bt.val:.4f} ({bt.avg:.4f})\tloss {loss.val:.3f} ({loss.avg:.3f})\t"
                       "prob {prob.val:.3f} ({prob.avg:.3f})\tGS {gs.val:.3f} ({gs.avg:.3f})\tlr {lr:.6f}".format(
-                          epoch, idx + 1, n_batch, bt=batch_time, loss=loss_meter, prob=prob_meter, gs=gs_meter, lr=lr))
+                          epoch, idx + 1, n_steps, bt=batch_time, loss=loss_meter, prob=prob_meter, gs=gs_meter, lr=lr))
         if sw is not None and (idx + 1) % opt.tb_freq == 0:
             sw.add_scalar("moco_loss", loss_meter.avg, global_step)
             sw.add_scalar("moco_prob", prob_meter.avg, global_step)
@@ -391,11 +416,7 @@ def main(args):
     torch.manual_seed(args.seed)
     torch.cuda.manual_seed(args.seed)
     args = option_update(args)
-    train_dataset = LoadBalanceGraphDataset(
-        rw_hops=args.rw_hops, restart_prob=args.restart_prob,
-        positional_embedding_size=args.positional_embedding_size, num_workers=args.num_workers,
-        num_samples=args.num_samples, dgl_graphs_file=build_graph(args, dev), num_copies=args.num_copies,
-        batch_size=args.batch_size, seed=args.seed, device=dev)
+    train_dataset = build_dataset(args, dev)
     model, model_ema = [
         GraphEncoder(positional_embedding_size=args.positional_embedding_size, max_node_freq=args.max_node_freq,
                      max_edge_freq=args.max_edge_freq, max_degree=args.max_degree,
