@@ -6,9 +6,7 @@
 #include <mutex>
 
 namespace gccb {
-#ifndef GCCB_EMU
 unsigned long long g_launch_count = 0;   // kernels enqueued by this library (bench.py: gpu_launches)
-#endif
 static thread_local char g_err[512] = "";
 
 void set_last_error(const char* fmt, ...) {
@@ -29,16 +27,24 @@ int check_launch(const char* what) {
 
 #ifndef GCCB_EMU
 // a library side stream with the caller stream's scheduling priority (a default-priority weight-gradient
-// stream starves behind queued eigensolver CTAs, DESIGN.md 5b), or the lowest priority on request
-static cudaStream_t create_stream_like(cudaStream_t like, bool lowest_priority) {
+// stream starves behind queued eigensolver CTAs, DESIGN.md 5b), the lowest priority, or one step above the
+// caller's (clamped to the device's greatest; a smaller number is a higher priority)
+static cudaStream_t create_stream_like(cudaStream_t like, SidePriority want) {
   int prio = 0;
-  if (lowest_priority || cudaStreamGetPriority(like, &prio) != cudaSuccess) { cudaGetLastError(); prio = 0; }
+  if (want == SidePriority::kLowest || cudaStreamGetPriority(like, &prio) != cudaSuccess) {
+    cudaGetLastError();
+    prio = 0;
+  } else if (want == SidePriority::kAboveCaller) {
+    int least = 0, greatest = 0;
+    if (cudaDeviceGetStreamPriorityRange(&least, &greatest) != cudaSuccess) cudaGetLastError();
+    else if (prio > greatest) --prio;
+  }
   cudaStream_t s = nullptr;
   cudaStreamCreateWithPriority(&s, cudaStreamNonBlocking, prio);
   return s;
 }
 
-StreamKit* stream_kit(cudaStream_t caller, int family, bool lowest_priority) {
+StreamKit* stream_kit(cudaStream_t caller, int family, SidePriority priority) {
   static StreamKit kits[16];
   static int nkits = 0;
   static std::mutex mu;
@@ -50,7 +56,7 @@ StreamKit* stream_kit(cudaStream_t caller, int family, bool lowest_priority) {
   StreamKit* k;
   if (nkits < 16) {
     k = &kits[nkits++];
-    for (int i = 0; i < 5; ++i) k->side[i] = create_stream_like(caller, lowest_priority);
+    for (int i = 0; i < 5; ++i) k->side[i] = create_stream_like(caller, priority);
     for (int i = 0; i < 24; ++i) cudaEventCreateWithFlags(&k->ev[i], cudaEventDisableTiming);
   } else {
     k = &kits[15];                                        // more caller streams than kits: share the last one
@@ -65,13 +71,7 @@ StreamKit* stream_kit(cudaStream_t caller, int family, bool lowest_priority) {
 
 extern "C" int gccb_version(void) { return GCCB_VERSION; }
 
-extern "C" unsigned long long gccb_launch_count(void) {
-#ifndef GCCB_EMU
-  return gccb::g_launch_count;
-#else
-  return 0;
-#endif
-}
+extern "C" unsigned long long gccb_launch_count(void) { return gccb::g_launch_count; }
 
 extern "C" const char* gccb_last_error(void) { return gccb::g_err; }
 

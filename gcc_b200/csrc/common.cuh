@@ -10,6 +10,11 @@
 // tests/emu/cuda_emu.h: CPU emulation used ONLY by the `-m "not gpu"` kernel-logic
 // tests; the product library is always built by nvcc without GCCB_EMU.
 #include "cuda_emu.h"
+// count kernel launches like the device build does (gccb_launch_count)
+namespace gccb { extern unsigned long long g_launch_count; }
+#undef GCCB_LAUNCH
+#define GCCB_LAUNCH(kern, grid, block, smem, stream, ...) \
+  (++gccb::g_launch_count, emu::launch(dim3(grid), dim3(block), (size_t)(smem), [=]() { kern(__VA_ARGS__); }))
 #else
 #include <cuda_runtime.h>
 #define GCCB_DYN_SMEM(type, name)                                   \
@@ -33,7 +38,9 @@ struct StreamKit {
   cudaStream_t side[5];
   cudaEvent_t ev[24];
 };
-StreamKit* stream_kit(cudaStream_t caller, int family, bool lowest_priority = false);
+// scheduling priority of a kit's side streams: the caller stream's, the lowest, or one step above the caller's
+enum class SidePriority { kCaller, kLowest, kAboveCaller };
+StreamKit* stream_kit(cudaStream_t caller, int family, SidePriority priority = SidePriority::kCaller);
 }  // namespace gccb
 #endif
 

@@ -118,64 +118,6 @@ gin_pred_wgrad_kernel(GinDims d, int B, gccb_gin_layout_t lay, const float* __re
   }
 }
 
-// dh_j[i] = dpool_j[gid[i]] + (has_da ? da[i] + sum_nbr da[nbr] : 0)      (width W)
-template <int W>
-__global__ void __launch_bounds__(256)
-gin_bwd_dh_kernel(const int32_t* __restrict__ node_off_v, int B, const int32_t* __restrict__ indptr,
-                  const int32_t* __restrict__ indices, const int32_t* __restrict__ graph_id,
-                  const float* __restrict__ dpool_j, int DW, const float* __restrict__ da, int has_da,
-                  float* __restrict__ dh) {
-  __shared__ float scratch[8 * W];
-  __shared__ int hub_rows[GCCB_HUB_QUEUE];
-  __shared__ int n_hub;
-  const int N = node_off_v[B];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  constexpr int V4 = W / 4, PERV = (V4 + 31) / 32;
-  // one warp per row, round-robin over the grid's warps, no barrier in the loop; hub rows are queued per CTA and
-  // gathered by its 8 warps together afterwards (see gin_agg_cast_kernel)
-  if (tid == 0) n_hub = 0;
-  __syncthreads();
-  for (int r = blockIdx.x * 8 + warp; r < N; r += gridDim.x * 8) {
-    const int beg = indptr[r], end = indptr[r + 1];
-    if (has_da && end - beg > GCCB_HUB_DEG) {
-      int slot = GCCB_HUB_QUEUE;
-      if (lane == 0) slot = atomicAdd(&n_hub, 1);
-      slot = __shfl_sync(0xffffffffu, slot, 0);
-      if (slot < GCCB_HUB_QUEUE) {
-        if (lane == 0) hub_rows[slot] = r;
-        continue;
-      }
-    }
-    const int g = graph_id[r];
-    float4 acc[PERV];
-#pragma unroll
-    for (int j = 0; j < PERV; ++j) {
-      const int v = lane + 32 * j;
-      acc[j] = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (v < V4) {
-        acc[j] = *reinterpret_cast<const float4*>(dpool_j + (size_t)g * DW + 4 * v);
-        if (has_da) {
-          const float4 x = *reinterpret_cast<const float4*>(da + (size_t)r * W + 4 * v);
-          acc[j].x += x.x; acc[j].y += x.y; acc[j].z += x.z; acc[j].w += x.w;
-        }
-      }
-    }
-    if (has_da) gather_range4<W>(da, indices, beg, end, lane, acc);
-#pragma unroll
-    for (int j = 0; j < PERV; ++j) {
-      const int v = lane + 32 * j;
-      if (v < V4) *reinterpret_cast<float4*>(dh + (size_t)r * W + 4 * v) = acc[j];
-    }
-  }
-  __syncthreads();
-  const int nh = min(n_hub, GCCB_HUB_QUEUE);
-  for (int hi = 0; hi < nh; ++hi) {
-    const int rh = hub_rows[hi];
-    const float s = gather_hub<W>(da, indices, indptr[rh], indptr[rh + 1], scratch);
-    if (tid < W) dh[(size_t)rh * W + tid] = dpool_j[(size_t)graph_id[rh] * DW + tid] + da[(size_t)rh * W + tid] + s;
-  }
-}
-
 // BN coefficient bundle in shared memory: mean | invstd | sc | sh   (4*H floats)
 struct BnC { const float *mean, *invstd, *sc, *sh; };
 __device__ __forceinline__ BnC bnc(const float* p, int H) { BnC b; b.mean = p; b.invstd = p + H; b.sc = p + 2 * H; b.sh = p + 3 * H; return b; }
@@ -192,11 +134,161 @@ __device__ __forceinline__ void chain_g4(float z2v, float dhv, const BnC& A, con
   *g4 = hb > 0.f ? dhv : 0.f;
 }
 
-// Column reductions for BN_b (mode 0: sum g4, sum g4*yhat) and BN_a (mode 1: sum g3, sum g3*z2hat)
+// dh_j[i] = dpool_j[gid[i]] + (has_da ? da[i] + sum_nbr da[nbr] : 0)      (width W)
+// BNB: also BN_b's backward reduction of the layer (sum g4, sum g4*yhat per column, chain_g4 from z2 and the
+// finished dh row) into redB_out, the quantities gin_bwd_reduce_kernel's BN_a pass and GEMM2 consume.
+template <int W, bool BNB>
+__global__ void __launch_bounds__(256)
+gin_bwd_dh_kernel(const int32_t* __restrict__ node_off_v, int B, const int32_t* __restrict__ indptr,
+                  const int32_t* __restrict__ indices, const int32_t* __restrict__ graph_id,
+                  const float* __restrict__ dpool_j, int DW, const float* __restrict__ da, int has_da,
+                  float* __restrict__ dh, const float* __restrict__ z2, const double* __restrict__ sums_a,
+                  const float* __restrict__ ga, const float* __restrict__ bea, const double* __restrict__ sums_b,
+                  const float* __restrict__ gb, const float* __restrict__ beb, float bn_eps,
+                  double* __restrict__ redB_out) {
+  __shared__ float scratch[8 * W];
+  __shared__ float coef[BNB ? 8 * W : 1];            // bn_a | bn_b bundles
+  __shared__ float red[BNB ? 9 * 2 * W : 1];         // [8 warps + hub rows][sum g4 | sum g4*yhat][W]
+  __shared__ int hub_rows[GCCB_HUB_QUEUE];
+  __shared__ int n_hub;
+  const int N = node_off_v[B];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  constexpr int V4 = W / 4, PERV = (V4 + 31) / 32;
+  // A warp pass finishes RPW rows, LW lanes per row (W = 64: two half-warps, W = 32: four quarter-warps, wider rows:
+  // one warp), rows dealt round-robin over the grid's warps, no barrier in the loop; hub rows are queued per CTA and
+  // gathered by its 8 warps together afterwards (see gin_agg_cast_kernel).  A lane owns the same columns in every
+  // row it finishes, so its BN_b partial sums stay in registers until one combine per CTA.
+  constexpr int LW = V4 < 32 ? V4 : 32, RPW = 32 / LW;
+  const int sub = lane / LW, vl = lane - sub * LW;
+  if (tid == 0) n_hub = 0;
+  if constexpr (BNB) {
+    bn_prepare(sums_a, N, W, ga, bea, bn_eps, coef, coef + W, coef + 2 * W, coef + 3 * W, nullptr, false, false, 0.f);
+    bn_prepare(sums_b, N, W, gb, beb, bn_eps, coef + 4 * W, coef + 5 * W, coef + 6 * W, coef + 7 * W, nullptr, false,
+               false, 0.f);
+  }
+  __syncthreads();
+  const BnC A = bnc(coef, W), Bc = bnc(coef + 4 * W, W);
+  float bs[PERV][4], bq[PERV][4];
+#pragma unroll
+  for (int j = 0; j < PERV; ++j)
+#pragma unroll
+    for (int k = 0; k < 4; ++k) bs[j][k] = bq[j][k] = 0.f;
+  for (int r0 = (blockIdx.x * 8 + warp) * RPW; r0 < N; r0 += gridDim.x * 8 * RPW) {
+    const int r = r0 + sub;
+    const bool live = r < N;
+    int beg = 0, end = 0;
+    if (live) { beg = indptr[r]; end = indptr[r + 1]; }
+    bool queued = false;
+    if (has_da) {                                    // every lane reaches the shuffle, whatever its row
+      const bool hub = live && end - beg > GCCB_HUB_DEG;
+      int slot = GCCB_HUB_QUEUE;
+      if (hub && vl == 0) slot = atomicAdd(&n_hub, 1);
+      slot = __shfl_sync(0xffffffffu, slot, sub * LW);
+      if (hub && slot < GCCB_HUB_QUEUE) {            // queue full: the lanes of the row gather it alone
+        if (vl == 0) hub_rows[slot] = r;
+        queued = true;
+      }
+    }
+    if (!live || queued) continue;
+    float4 zv[PERV];                                 // BN_b's input, loaded before the gather so that it overlaps it
+    if constexpr (BNB) {
+#pragma unroll
+      for (int j = 0; j < PERV; ++j) {
+        const int v = vl + 32 * j;
+        if (v < V4) zv[j] = *reinterpret_cast<const float4*>(z2 + (size_t)r * W + 4 * v);
+      }
+    }
+    const int g = graph_id[r];
+    float4 acc[PERV];
+#pragma unroll
+    for (int j = 0; j < PERV; ++j) {
+      const int v = vl + 32 * j;
+      acc[j] = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (v < V4) {
+        acc[j] = *reinterpret_cast<const float4*>(dpool_j + (size_t)g * DW + 4 * v);
+        if (has_da) {
+          const float4 x = *reinterpret_cast<const float4*>(da + (size_t)r * W + 4 * v);
+          acc[j].x += x.x; acc[j].y += x.y; acc[j].z += x.z; acc[j].w += x.w;
+        }
+      }
+    }
+    if (has_da) gather_range4<W>(da, indices, beg, end, vl, acc);
+#pragma unroll
+    for (int j = 0; j < PERV; ++j) {
+      const int v = vl + 32 * j;
+      if (v < V4) {
+        *reinterpret_cast<float4*>(dh + (size_t)r * W + 4 * v) = acc[j];
+        if constexpr (BNB) {
+          const float zz[4] = {zv[j].x, zv[j].y, zv[j].z, zv[j].w}, dd[4] = {acc[j].x, acc[j].y, acc[j].z, acc[j].w};
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            float ya, yhat, g4;
+            chain_g4(zz[k], dd[k], A, Bc, 4 * v + k, &ya, &yhat, &g4);
+            bs[j][k] += g4;
+            bq[j][k] = fmaf(g4, yhat, bq[j][k]);
+          }
+        }
+      }
+    }
+  }
+  __syncthreads();
+  float hs = 0.f, hq = 0.f;                          // hub rows: thread tid < W owns column tid
+  const int nh = min(n_hub, GCCB_HUB_QUEUE);
+  for (int hi = 0; hi < nh; ++hi) {
+    const int rh = hub_rows[hi];
+    const float s = gather_hub<W>(da, indices, indptr[rh], indptr[rh + 1], scratch);
+    if (tid < W) {
+      const float dv = dpool_j[(size_t)graph_id[rh] * DW + tid] + da[(size_t)rh * W + tid] + s;
+      dh[(size_t)rh * W + tid] = dv;
+      if constexpr (BNB) {
+        float ya, yhat, g4;
+        chain_g4(z2[(size_t)rh * W + tid], dv, A, Bc, tid, &ya, &yhat, &g4);
+        hs += g4;
+        hq = fmaf(g4, yhat, hq);
+      }
+    }
+  }
+  if constexpr (BNB) {
+#pragma unroll
+    for (int o = LW; o < 32; o <<= 1)                // the RPW rows of a warp pass share their columns
+#pragma unroll
+      for (int j = 0; j < PERV; ++j)
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          bs[j][k] += __shfl_xor_sync(0xffffffffu, bs[j][k], o);
+          bq[j][k] += __shfl_xor_sync(0xffffffffu, bq[j][k], o);
+        }
+#pragma unroll
+    for (int j = 0; j < PERV; ++j) {
+      const int v = vl + 32 * j;
+      if (sub == 0 && v < V4) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          red[(warp * 2 + 0) * W + 4 * v + k] = bs[j][k];
+          red[(warp * 2 + 1) * W + 4 * v + k] = bq[j][k];
+        }
+      }
+    }
+    if (tid < W) {
+      red[16 * W + tid] = hs;
+      red[17 * W + tid] = hq;
+    }
+    __syncthreads();
+    for (int idx = tid; idx < 2 * W; idx += 256) {
+      const int which = idx / W, c = idx - which * W;
+      float t = 0.f;
+#pragma unroll
+      for (int w = 0; w < 9; ++w) t += red[(w * 2 + which) * W + c];
+      atomicAdd(&redB_out[which * W + c], (double)t);
+    }
+  }
+}
+
+// Column reductions for BN_a (sum g3, sum g3*z2hat); BN_b's (sum g4, sum g4*yhat) come from gin_bwd_dh_kernel
 // thread -> 4 consecutive columns of every RP-th row, two rows (4 x 16-byte loads) in flight per thread
 template <int H>
 __global__ void __launch_bounds__(256)
-gin_bwd_reduce_kernel(int mode, const int32_t* __restrict__ node_off_v, int B,
+gin_bwd_reduce_kernel(const int32_t* __restrict__ node_off_v, int B,
                       const float* __restrict__ z2, const float* __restrict__ dh,
                       const double* __restrict__ sums_a, const float* __restrict__ ga,
                       const float* __restrict__ bea, const double* __restrict__ sums_b,
@@ -214,11 +306,9 @@ gin_bwd_reduce_kernel(int mode, const int32_t* __restrict__ node_off_v, int B,
   constexpr int TPR = H / 4, RP = 256 / TPR;
   const int c4 = (tid % TPR) * 4, rsub = tid / TPR;
   const float invN = N > 0 ? 1.0f / (float)N : 0.f;
-  float m_g4[4] = {0.f, 0.f, 0.f, 0.f}, m_g4y[4] = {0.f, 0.f, 0.f, 0.f};
-  if (mode == 1) {
+  float m_g4[4], m_g4y[4];
 #pragma unroll
-    for (int k = 0; k < 4; ++k) { m_g4[k] = (float)(redB_in[c4 + k] * invN); m_g4y[k] = (float)(redB_in[H + c4 + k] * invN); }
-  }
+  for (int k = 0; k < 4; ++k) { m_g4[k] = (float)(redB_in[c4 + k] * invN); m_g4y[k] = (float)(redB_in[H + c4 + k] * invN); }
   float s[4] = {0.f, 0.f, 0.f, 0.f}, q[4] = {0.f, 0.f, 0.f, 0.f};
   const int stride = gridDim.x * RP;
   for (int r = blockIdx.x * RP + rsub; r < N; r += 2 * stride) {
@@ -239,16 +329,11 @@ gin_bwd_reduce_kernel(int mode, const int32_t* __restrict__ node_off_v, int B,
           const int c = c4 + k;
           float ya, yhat, g4;
           chain_g4(zz[k], dd[k], A, Bc, c, &ya, &yhat, &g4);
-          if (mode == 0) {
-            s[k] += g4;
-            q[k] = fmaf(g4, yhat, q[k]);
-          } else {
-            const float dy = Bc.sc[c] * (g4 - m_g4[k] - yhat * m_g4y[k]);
-            const float g3 = ya > 0.f ? dy : 0.f;
-            const float z2hat = (zz[k] - A.mean[c]) * A.invstd[c];
-            s[k] += g3;
-            q[k] = fmaf(g3, z2hat, q[k]);
-          }
+          const float dy = Bc.sc[c] * (g4 - m_g4[k] - yhat * m_g4y[k]);
+          const float g3 = ya > 0.f ? dy : 0.f;
+          const float z2hat = (zz[k] - A.mean[c]) * A.invstd[c];
+          s[k] += g3;
+          q[k] = fmaf(g3, z2hat, q[k]);
         }
       }
     }
@@ -615,16 +700,20 @@ static int run_backward(const BwdArgs& a) {
   const uint32_t keep = (uint32_t)fmin((1.0 - (double)d.drop_p) * 4294967296.0, 4294967295.0);
   // The input-gradient chain (dh -> BN reductions -> GEMM2 -> GEMM1 -> next layer) is the critical
   // path; weight / BatchNorm / head gradients only consume its by-products, so they run on a side
-  // stream (event fork per layer, one join at the end).  g1/dz2 alternate between two buffers so
-  // that layer l-1 may overwrite nothing the side stream still reads from layer l; layer l-2
-  // waits for the side work of layer l before reusing its buffers.
+  // stream (two event forks per layer, after GEMM2 and after GEMM1, one join at the end).  g1/dz2
+  // alternate between two buffers so that layer l-1 may overwrite nothing the side stream still reads
+  // from layer l; layer l-2 waits for the side work of layer l before reusing its buffers.
 #ifndef GCCB_EMU
-  StreamKit* kit = stream_kit((cudaStream_t)a.stream, 1);
+  // The side stream runs one step above the caller's priority: its kernels are short (one wave of CTAs), and
+  // at equal priority they queued behind the next chain kernel's CTAs, so the side stream fell behind and the
+  // final join (before the optimiser) waited for the last layers' weight gradients.
+  StreamKit* kit = stream_kit((cudaStream_t)a.stream, 2, SidePriority::kAboveCaller);
   cudaStream_t main_s = (cudaStream_t)a.stream;
   gccb_stream_t side = kit->side[0];
   cudaEvent_t* ev_main = kit->ev;                          // [0..7]  main -> side, per layer
   cudaEvent_t* ev_side = kit->ev + 8;                      // [8..15] side -> main, per layer
   cudaEvent_t ev_head = kit->ev[16], ev_join = kit->ev[17];
+  cudaEvent_t ev_gemm2 = kit->ev[18];                      // main -> side after GEMM2, re-recorded per layer
 #else
   gccb_stream_t side = a.stream;
 #endif
@@ -656,14 +745,13 @@ static int run_backward(const BwdArgs& a) {
     double* rA = red + (size_t)(l * 3 + 1) * 2 * H;
     double* rB = red + (size_t)(l * 3 + 2) * 2 * H;
     // dh_j = dpool_j broadcast + (I + A) da_{j}   (da of the layer above; none for the top)
-    auto kdh = gin_bwd_dh_kernel<H>;
+    // and BN_b's backward reduction (rB) of this layer
+    auto kdh = gin_bwd_dh_kernel<H, true>;
     GCCB_LAUNCH(kdh, (tiles < 1184 ? tiles : 1184), 256, 0, a.stream, node_off_v, B, indptr, indices, graph_id,
-                (const float*)(dpool + (size_t)j * B * DW), DW, (const float*)da, j < d.L - 1 ? 1 : 0, dh);
+                (const float*)(dpool + (size_t)j * B * DW), DW, (const float*)da, j < d.L - 1 ? 1 : 0, dh, z2, sa,
+                P + a.lay.bna_w[l], P + a.lay.bna_b[l], sb, P + a.lay.bnb_w[l], P + a.lay.bnb_b[l], d.bn_eps, rB);
     auto kred = gin_bwd_reduce_kernel<H>;
-    GCCB_LAUNCH(kred, grid, 256, 0, a.stream, 0, node_off_v, B, z2, (const float*)dh, sa, P + a.lay.bna_w[l],
-                P + a.lay.bna_b[l], sb, P + a.lay.bnb_w[l], P + a.lay.bnb_b[l], d.bn_eps,
-                (const double*)rB, rB);
-    GCCB_LAUNCH(kred, grid, 256, 0, a.stream, 1, node_off_v, B, z2, (const float*)dh, sa, P + a.lay.bna_w[l],
+    GCCB_LAUNCH(kred, grid, 256, 0, a.stream, node_off_v, B, z2, (const float*)dh, sa, P + a.lay.bna_w[l],
                 P + a.lay.bna_b[l], sb, P + a.lay.bnb_w[l], P + a.lay.bnb_b[l], d.bn_eps,
                 (const double*)rB, rA);
 #ifndef GCCB_EMU
@@ -678,6 +766,25 @@ static int run_backward(const BwdArgs& a) {
                   P + a.lay.bnb_b[l], d.bn_eps, (const double*)rB, (const double*)rA, P + a.lay.w2[l], dz2,
                   g1, r1);
     }
+#ifndef GCCB_EMU
+    cudaEventRecord(ev_gemm2, main_s);
+    cudaStreamWaitEvent((cudaStream_t)side, ev_gemm2, 0);
+#endif
+    // side stream, as soon as GEMM2 has left dz2 and the last BatchNorm reduction (r1): dW2 = dz2^T x1
+    // (x1 = relu(bn1(z1))) and the three BatchNorm affine gradients
+    {
+      dim3 gr(GCCB_WG_CHUNKS, ((H + 63) / 64) * ((H + 63) / 64));
+      GCCB_LAUNCH(gin_wgrad_kernel, gr, 256, 0, side, node_off_v, B, H, H, (const float*)dz2, z1, s1,
+                  P + a.lay.bn1_w[l], P + a.lay.bn1_b[l], d.bn_eps, part);
+      GCCB_LAUNCH(gin_wgrad_reduce_kernel, (H * H + H + 255) / 256, 256, 0, side, H, H, H,
+                  (const float*)part, G + a.lay.w2[l], G + a.lay.b2[l]);
+    }
+    GCCB_LAUNCH(gin_bn_grads_kernel, (H + 127) / 128, 128, 0, side, H, (const double*)rB,
+                G + a.lay.bnb_w[l], G + a.lay.bnb_b[l]);
+    GCCB_LAUNCH(gin_bn_grads_kernel, (H + 127) / 128, 128, 0, side, H, (const double*)rA,
+                G + a.lay.bna_w[l], G + a.lay.bna_b[l]);
+    GCCB_LAUNCH(gin_bn_grads_kernel, (H + 127) / 128, 128, 0, side, H, (const double*)r1,
+                G + a.lay.bn1_w[l], G + a.lay.bn1_b[l]);
     const int KQ1 = gin_in_width(d, l), inf = gin_in_features(d, l);
     if (l == 0) {
       auto k = gin_bwd_gemm1_kernel<GCCB_DINP, H>;
@@ -696,33 +803,22 @@ static int run_backward(const BwdArgs& a) {
     cudaEventRecord(ev_main[l], main_s);
     cudaStreamWaitEvent((cudaStream_t)side, ev_main[l], 0);
 #endif
-    // weight gradients (side stream): dW2 = dz2^T x1 (x1 = relu(bn1(z1))), dW1 = dz1^T a
+    // side stream, once GEMM1 has turned g1 into dz1: dW1 = dz1^T a
     {
-      dim3 gr(GCCB_WG_CHUNKS, ((H + 63) / 64) * ((H + 63) / 64));
-      GCCB_LAUNCH(gin_wgrad_kernel, gr, 256, 0, side, node_off_v, B, H, H, (const float*)dz2, z1, s1,
-                  P + a.lay.bn1_w[l], P + a.lay.bn1_b[l], d.bn_eps, part);
-      GCCB_LAUNCH(gin_wgrad_reduce_kernel, (H * H + H + 255) / 256, 256, 0, side, H, H, H,
-                  (const float*)part, G + a.lay.w2[l], G + a.lay.b2[l]);
       dim3 gr1(GCCB_WG_CHUNKS, ((H + 63) / 64) * ((KQ1 + 63) / 64));
       GCCB_LAUNCH(gin_wgrad_kernel, gr1, 256, 0, side, node_off_v, B, H, KQ1, (const float*)g1, a_l,
                   (const double*)nullptr, (const float*)nullptr, (const float*)nullptr, d.bn_eps, part);
       GCCB_LAUNCH(gin_wgrad_reduce_kernel, (H * KQ1 + H + 255) / 256, 256, 0, side, H, KQ1, inf,
                   (const float*)part, G + a.lay.w1[l], G + a.lay.b1[l]);
     }
-    GCCB_LAUNCH(gin_bn_grads_kernel, (H + 127) / 128, 128, 0, side, H, (const double*)rB,
-                G + a.lay.bnb_w[l], G + a.lay.bnb_b[l]);
-    GCCB_LAUNCH(gin_bn_grads_kernel, (H + 127) / 128, 128, 0, side, H, (const double*)rA,
-                G + a.lay.bna_w[l], G + a.lay.bna_b[l]);
-    GCCB_LAUNCH(gin_bn_grads_kernel, (H + 127) / 128, 128, 0, side, H, (const double*)r1,
-                G + a.lay.bn1_w[l], G + a.lay.bn1_b[l]);
 #ifndef GCCB_EMU
     cudaEventRecord(ev_side[l], (cudaStream_t)side);
 #endif
   }
   // layer-0 input gradient -> degree embedding
-  auto kdh0 = gin_bwd_dh_kernel<GCCB_DINP>;
+  auto kdh0 = gin_bwd_dh_kernel<GCCB_DINP, false>;
   GCCB_LAUNCH(kdh0, (tiles < 1184 ? tiles : 1184), 256, 0, a.stream, node_off_v, B, indptr, indices, graph_id, (const float*)dpool, DW,
-              (const float*)da, 1, dh);
+              (const float*)da, 1, dh, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0.f, nullptr);
   {
     size_t sm = (size_t)(d.maxdeg + 1) * d.D * sizeof(float);
     auto k = gin_bwd_emb_kernel;
@@ -990,13 +1086,12 @@ static int run_backward_tc(const BwdArgs& a) {
     const __nv_bfloat16* w1t = w1b + (size_t)H * KW + (size_t)H * H;
     const __nv_bfloat16* w2t = w1t + (size_t)KW * H;
     float* c1 = coef1 + (size_t)l * 2 * H;
-    auto kdh = gin_bwd_dh_kernel<H>;
+    auto kdh = gin_bwd_dh_kernel<H, true>;                // dh and BN_b's backward reduction (rB)
     GCCB_LAUNCH(kdh, (tiles < 1184 ? tiles : 1184), 256, 0, a.stream, node_off_v, B, indptr, indices, graph_id,
-                (const float*)(dpool + (size_t)j * B * DW), DW, (const float*)da, j < d.L - 1 ? 1 : 0, dh);
+                (const float*)(dpool + (size_t)j * B * DW), DW, (const float*)da, j < d.L - 1 ? 1 : 0, dh, z2, sa,
+                P + a.lay.bna_w[l], P + a.lay.bna_b[l], sb, P + a.lay.bnb_w[l], P + a.lay.bnb_b[l], d.bn_eps, rB);
     auto kred = gin_bwd_reduce_kernel<H>;
-    GCCB_LAUNCH(kred, grid, 256, 0, a.stream, 0, node_off_v, B, z2, (const float*)dh, sa, P + a.lay.bna_w[l],
-                P + a.lay.bna_b[l], sb, P + a.lay.bnb_w[l], P + a.lay.bnb_b[l], d.bn_eps, (const double*)rB, rB);
-    GCCB_LAUNCH(kred, grid, 256, 0, a.stream, 1, node_off_v, B, z2, (const float*)dh, sa, P + a.lay.bna_w[l],
+    GCCB_LAUNCH(kred, grid, 256, 0, a.stream, node_off_v, B, z2, (const float*)dh, sa, P + a.lay.bna_w[l],
                 P + a.lay.bna_b[l], sb, P + a.lay.bnb_w[l], P + a.lay.bnb_b[l], d.bn_eps, (const double*)rB, rA);
     if (l + 2 <= d.L - 2) cudaStreamWaitEvent(main_s, ev_side[l + 2], 0);   // g1 / dz2 [l&1] free again
     // the side stream of the layer above still reads dz16's transposed copies, not dz16 itself: no wait needed
@@ -1034,9 +1129,9 @@ static int run_backward_tc(const BwdArgs& a) {
                 G + a.lay.bn1_w[l], G + a.lay.bn1_b[l]);
     cudaEventRecord(ev_side[l], side);
   }
-  auto kdh0 = gin_bwd_dh_kernel<GCCB_DINP>;
+  auto kdh0 = gin_bwd_dh_kernel<GCCB_DINP, false>;
   GCCB_LAUNCH(kdh0, (tiles < 1184 ? tiles : 1184), 256, 0, a.stream, node_off_v, B, indptr, indices, graph_id, (const float*)dpool, DW,
-              (const float*)da, 1, dh);
+              (const float*)da, 1, dh, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0.f, nullptr);
   {
     size_t sm = (size_t)(d.maxdeg + 1) * d.D * sizeof(float);
     auto k = gin_bwd_emb_kernel;

@@ -1,5 +1,7 @@
 // gin_common.cuh -- layouts and tile helpers shared by the GIN forward / backward kernels.
 #pragma once
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace gccb {
@@ -207,9 +209,29 @@ __device__ __forceinline__ void bn_prepare(const double* __restrict__ sums, int 
 #endif
 #define GCCB_GPB 8            // graphs per CTA of the pooled prediction heads (one warp per graph at the end)
 #define GCCB_HUB_QUEUE 64     // hub rows a CTA of the barrier-free gather kernels defers to its cooperative pass
-template <int W>
+
+// Transform applied to every element a scalar gather reads: xf(x, j) for the column lane + 32 j of the lane.
+struct GatherIdentity {
+  __device__ __forceinline__ float operator()(float x, int) const { return x; }
+};
+
+// h = relu(bn_b(relu(bn_a(z2)))): the tail of a GIN layer (gin.py:55-57, :219-220) from its two BatchNorms'
+// scale / shift, in the order gin_bn_tail_kernel applies it
+__device__ __forceinline__ float bn_tail_h(float z, float sca, float sha, float scb, float shb) {
+  return fmaxf(fmaf(fmaxf(fmaf(z, sca, sha), 0.f), scb, shb), 0.f);
+}
+
+// bn_tail_h with the coefficients of the lane's columns lane + 32 j held in registers
+template <int PER>
+struct BnTailXf {
+  float sca[PER], sha[PER], scb[PER], shb[PER];
+  __device__ __forceinline__ float operator()(float z, int j) const { return bn_tail_h(z, sca[j], sha[j], scb[j], shb[j]); }
+};
+
+template <int W, class Xf = GatherIdentity>
 __device__ __forceinline__ void gather_range(const float* __restrict__ src, const int32_t* __restrict__ indices,
-                                             int beg, int end, int lane, float (&acc)[(W + 31) / 32]) {
+                                             int beg, int end, int lane, float (&acc)[(W + 31) / 32],
+                                             const Xf& xf = Xf()) {
   constexpr int PER = (W + 31) / 32;
   int e = beg;
   for (; e + 7 < end; e += 8) {
@@ -222,7 +244,7 @@ __device__ __forceinline__ void gather_range(const float* __restrict__ src, cons
       if (c < W) {
         float x[8];
 #pragma unroll
-        for (int k = 0; k < 8; ++k) x[k] = src[(size_t)u[k] * W + c];
+        for (int k = 0; k < 8; ++k) x[k] = xf(src[(size_t)u[k] * W + c], j);
         acc[j] += ((x[0] + x[1]) + (x[2] + x[3])) + ((x[4] + x[5]) + (x[6] + x[7]));
       }
     }
@@ -232,7 +254,7 @@ __device__ __forceinline__ void gather_range(const float* __restrict__ src, cons
 #pragma unroll
     for (int j = 0; j < PER; ++j) {
       const int c = lane + 32 * j;
-      if (c < W) acc[j] += src[(size_t)u * W + c];
+      if (c < W) acc[j] += xf(src[(size_t)u * W + c], j);
     }
   }
 }
@@ -277,9 +299,9 @@ __device__ __forceinline__ void gather_range4(const float* __restrict__ src, con
 // Hub row: the 8 warps of a 256-thread CTA each gather a contiguous eighth of the neighbour list;
 // partial sums meet in `scratch` [8][W]; on return (after the internal barriers) every thread
 // c < W holds the full neighbour sum of column c in the return value.  All 256 threads must call.
-template <int W>
+template <int W, class Xf = GatherIdentity>
 __device__ __forceinline__ float gather_hub(const float* __restrict__ src, const int32_t* __restrict__ indices,
-                                            int beg, int end, float* scratch) {
+                                            int beg, int end, float* scratch, const Xf& xf = Xf()) {
   constexpr int PER = (W + 31) / 32;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int len = end - beg, per = (len + 7) / 8;
@@ -287,7 +309,7 @@ __device__ __forceinline__ float gather_hub(const float* __restrict__ src, const
   float acc[PER];
 #pragma unroll
   for (int j = 0; j < PER; ++j) acc[j] = 0.f;
-  gather_range<W>(src, indices, b, e > b ? e : b, lane, acc);
+  gather_range<W>(src, indices, b, e > b ? e : b, lane, acc, xf);
 #pragma unroll
   for (int j = 0; j < PER; ++j) {
     const int c = lane + 32 * j;

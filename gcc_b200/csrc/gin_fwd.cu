@@ -10,7 +10,7 @@
 //   x1 = relu(bn1(z1))          (applied on load of GEMM2's A tile)
 //   z2 = x1 W2^T + b2           -> statistics
 //   y  = relu(bn_a(z2))         -> statistics (needs the full-batch mean of y)
-//   h' = relu(bn_b(y))
+//   h' = relu(bn_b(y))          (SIMT path: applied by h's readers, the next layer's gather or the pooling)
 // Every "-> statistics" is a column reduction over all N rows of the view, i.e. a
 // grid-wide dependency; kernel boundaries provide it.  Round 1 uses fp32 SIMT tiles
 // (bit-level agreement with an fp32 reference matters more than tensor-pipe speed
@@ -47,26 +47,66 @@ gin_build_x0_kernel(GinDims d, const int32_t* __restrict__ node_off_v, int B,
   }
 }
 
+// The last two BatchNorms of a GIN layer, h = relu(bn_b(relu(bn_a(z2)))), for the kernels that apply them where
+// h is read (the next layer's gather, or the pooling after the last layer) and leave h in the stash (h_out).
+struct BnTailArgs {
+  const double* sums_a;
+  const float *ga, *bea;
+  float* running_a;
+  const double* sums_b;
+  const float *gb, *beb;
+  float* running_b;
+  float bn_eps, momentum;
+  int use_running, update_running;
+  float* h_out;
+};
+
+// coef_a / coef_b: mean | invstd | sc | sh (4 H floats each).  BN_a's running statistics were updated by
+// gin_bn_tail_kernel mode 0; BN_b's are updated here, by block 0 only (bn_prepare), once per forward.
+__device__ __forceinline__ void bn_tail_prepare(const BnTailArgs& t, int N, int H, float* coef_a, float* coef_b) {
+  bn_prepare(t.sums_a, N, H, t.ga, t.bea, t.bn_eps, coef_a, coef_a + H, coef_a + 2 * H, coef_a + 3 * H, t.running_a,
+             t.use_running != 0, false, t.momentum);
+  bn_prepare(t.sums_b, N, H, t.gb, t.beb, t.bn_eps, coef_b, coef_b + H, coef_b + 2 * H, coef_b + 3 * H, t.running_b,
+             t.use_running != 0, t.update_running != 0, t.momentum);
+}
+
 // K1: a = h + sum_nbr h ; z1 = a W1^T + b1 ; column statistics of z1.
-template <int KIN, int H>
+// BN_IN: `h` is the layer below's z2, and every element read becomes h = relu(bn_b(relu(bn_a(z2)))) (`tail`);
+// the warp (or, for a hub row, the CTA) that owns row r also writes h_r to tail.h_out.
+template <int KIN, int H, bool BN_IN>
 __global__ void __launch_bounds__(256)
 gin_agg_gemm1_kernel(const int32_t* __restrict__ node_off_v, int B, const int32_t* __restrict__ indptr,
                      const int32_t* __restrict__ indices, const float* __restrict__ h,
                      const float* __restrict__ W1, int in_features, const float* __restrict__ b1,
                      float eps_gin, float* __restrict__ a_out, float* __restrict__ z1,
-                     double* __restrict__ sums) {
+                     double* __restrict__ sums, BnTailArgs tail) {
   GCCB_DYN_SMEM(float, smem);
   constexpr int LDA = KIN + 1;
+  constexpr int PER = (KIN + 31) / 32;
   float* As = smem;                          // [64][KIN+1]
   float* Ws = As + GCCB_TILE_ROWS * LDA;     // [KC][H+4]
   float* red = Ws + GCCB_KC * (H + 4);       // [2][16][H]; also the hub-row scratch [8][KIN]
+  float* coef = red + 2 * 16 * H;            // BN_IN: bn_a | bn_b coefficients (8 H)
   __shared__ int hub_rows[GCCB_TILE_ROWS];
   __shared__ int n_hub;
   static_assert(8 * KIN <= 2 * 16 * H, "hub scratch must fit in the statistics scratch");
+  static_assert(!BN_IN || KIN == H, "the BatchNorm tail is applied to a hidden-width input");
   const int N = node_off_v[B];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int tx = tid & 15, ty = tid >> 4;
   using TC = TileCols<H>;
+  using Xf = typename std::conditional<BN_IN, BnTailXf<PER>, GatherIdentity>::type;
+  Xf xf;
+  if constexpr (BN_IN) {
+    bn_tail_prepare(tail, N, H, coef, coef + 4 * H);
+    __syncthreads();
+#pragma unroll
+    for (int j = 0; j < PER; ++j) {
+      const int c = lane + 32 * j;            // KIN == H is a multiple of 32
+      xf.sca[j] = coef[2 * H + c]; xf.sha[j] = coef[3 * H + c];
+      xf.scb[j] = coef[6 * H + c]; xf.shb[j] = coef[7 * H + c];
+    }
+  }
   for (int tile = blockIdx.x; tile * GCCB_TILE_ROWS < N; tile += gridDim.x) {
     const int row0 = tile * GCCB_TILE_ROWS;
     __syncthreads();                                   // As free (previous tile consumed)
@@ -76,7 +116,6 @@ gin_agg_gemm1_kernel(const int32_t* __restrict__ node_off_v, int B, const int32_
     __syncthreads();
     for (int rr = warp; rr < GCCB_TILE_ROWS; rr += 8) {
       const int r = row0 + rr;
-      constexpr int PER = (KIN + 31) / 32;
       float acc[PER];
 #pragma unroll
       for (int j = 0; j < PER; ++j) acc[j] = 0.f;
@@ -89,9 +128,13 @@ gin_agg_gemm1_kernel(const int32_t* __restrict__ node_off_v, int B, const int32_
 #pragma unroll
         for (int j = 0; j < PER; ++j) {
           int c = lane + 32 * j;
-          if (c < KIN) acc[j] = (1.0f + eps_gin) * h[(size_t)r * KIN + c];
+          if (c < KIN) {
+            const float hv = xf(h[(size_t)r * KIN + c], j);
+            if (BN_IN) tail.h_out[(size_t)r * KIN + c] = hv;
+            acc[j] = (1.0f + eps_gin) * hv;
+          }
         }
-        gather_range<KIN>(h, indices, beg, end, lane, acc);
+        gather_range<KIN>(h, indices, beg, end, lane, acc, xf);
       }
 #pragma unroll
       for (int j = 0; j < PER; ++j) {
@@ -105,9 +148,14 @@ gin_agg_gemm1_kernel(const int32_t* __restrict__ node_off_v, int B, const int32_
     __syncthreads();
     for (int hi = 0; hi < n_hub; ++hi) {
       const int rr = hub_rows[hi], r = row0 + rr;
-      const float s = gather_hub<KIN>(h, indices, indptr[r], indptr[r + 1], red);
+      const float s = gather_hub<KIN>(h, indices, indptr[r], indptr[r + 1], red, xf);
       if (tid < KIN) {
-        const float v = (1.0f + eps_gin) * h[(size_t)r * KIN + tid] + s;
+        float hv = h[(size_t)r * KIN + tid];
+        if (BN_IN) {
+          hv = bn_tail_h(hv, coef[2 * H + tid], coef[3 * H + tid], coef[6 * H + tid], coef[7 * H + tid]);
+          tail.h_out[(size_t)r * KIN + tid] = hv;
+        }
+        const float v = (1.0f + eps_gin) * hv + s;
         As[rr * LDA + tid] = v;
         a_out[(size_t)r * KIN + tid] = v;
       }
@@ -186,7 +234,8 @@ gin_bn_gemm2_kernel(const int32_t* __restrict__ node_off_v, int B, const float* 
 }
 
 // K3: y = relu(bn_a(z2)); column statistics of y.   (elementwise + reduction)
-// K4 (mode 1): h' = relu(bn_b(y)) written out.
+// K4 (mode 1): h' = relu(bn_b(y)) written out -- tensor-core forward only; the SIMT forward applies BN_b where
+// h' is read (gin_agg_gemm1_kernel of the next layer, gin_pool_kernel after the last one).
 // One kernel, two modes: mode 0 accumulates sums of y; mode 1 writes h'.
 template <int H>
 __global__ void __launch_bounds__(256)
@@ -284,14 +333,18 @@ gin_bn_tail_kernel(int mode, const int32_t* __restrict__ node_off_v, int B,
 // tiles so that a 3,000-node ego-net does not serialise on one CTA: each thread owns a column and a
 // run of consecutive rows, accumulates while the graph id stays the same and flushes with a float64
 // atomic (same policy as the BatchNorm statistics).  pool_acc is zeroed with the statistics.
+// z2_last != null: the last layer's h is not in the stash yet; it is h = relu(bn_b(relu(bn_a(z2_last)))) (`tail`),
+// pooled and written to tail.h_out here.
 template <int H>
 __global__ void __launch_bounds__(256)
 gin_pool_kernel(int L, const int32_t* __restrict__ node_off_v, int B, const int32_t* __restrict__ graph_id,
                 const float* __restrict__ x0, const float* const* __restrict__ h_layers, int PW,
-                double* __restrict__ pool_acc) {
+                double* __restrict__ pool_acc, const float* __restrict__ z2_last, BnTailArgs tail) {
   __shared__ int gid[GCCB_TILE_ROWS];
+  __shared__ float coef_a[4 * H], coef_b[4 * H];
   const int N = node_off_v[B];
   const int tid = threadIdx.x;
+  if (z2_last) bn_tail_prepare(tail, N, H, coef_a, coef_b);
   for (int tile = blockIdx.x; tile * GCCB_TILE_ROWS < N; tile += gridDim.x) {
     const int row0 = tile * GCCB_TILE_ROWS;
     __syncthreads();
@@ -301,7 +354,8 @@ gin_pool_kernel(int L, const int32_t* __restrict__ node_off_v, int B, const int3
       // thread = (row group, float4 column): 128-bit loads, GCCB_TILE_ROWS / RG rows each, all of them in flight
       // (a scalar column per thread with 64 dependent-issue loads ran this pass at 0.9 TB/s at hidden 256)
       const int W = l == 0 ? GCCB_DINP : H;
-      const float* src = l == 0 ? x0 : h_layers[l - 1];
+      const bool xf = l == L - 1 && z2_last;             // W == H
+      const float* src = l == 0 ? x0 : xf ? z2_last : h_layers[l - 1];
       if (W < 128) {
         // narrow rows: one column per thread, 256 / W row groups (fewer, longer runs = fewer atomics)
         const int RGs = 256 / W > 0 ? 256 / W : 1;
@@ -311,11 +365,18 @@ gin_pool_kernel(int L, const int32_t* __restrict__ node_off_v, int B, const int3
         const int rbs = rgs * pers;
         int g_run = gid[rbs];
         float acc = 0.f;
+        float sca = 0.f, sha = 0.f, scb = 0.f, shb = 0.f;
+        if (xf) { sca = coef_a[2 * H + c]; sha = coef_a[3 * H + c]; scb = coef_b[2 * H + c]; shb = coef_b[3 * H + c]; }
 #pragma unroll 8
         for (int k = 0; k < pers; ++k) {
           const int g = gid[rbs + k];
           if (g < 0) break;
-          const float x = src[(size_t)(row0 + rbs + k) * W + c];
+          const size_t e = (size_t)(row0 + rbs + k) * W + c;
+          float x = src[e];
+          if (xf) {
+            x = bn_tail_h(x, sca, sha, scb, shb);
+            tail.h_out[e] = x;
+          }
           if (g != g_run) {
             atomicAdd(&pool_acc[((size_t)l * B + g_run) * PW + c], (double)acc);
             acc = 0.f;
@@ -334,6 +395,15 @@ gin_pool_kernel(int L, const int32_t* __restrict__ node_off_v, int B, const int3
       const int rb = rg * per;
       int g_run = gid[rb];
       float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+      float sca[4] = {0.f, 0.f, 0.f, 0.f}, sha[4] = {0.f, 0.f, 0.f, 0.f};
+      float scb[4] = {0.f, 0.f, 0.f, 0.f}, shb[4] = {0.f, 0.f, 0.f, 0.f};
+      if (xf) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          sca[k] = coef_a[2 * H + 4 * v + k]; sha[k] = coef_a[3 * H + 4 * v + k];
+          scb[k] = coef_b[2 * H + 4 * v + k]; shb[k] = coef_b[3 * H + 4 * v + k];
+        }
+      }
       auto flush = [&](int g) {
         double* dst = &pool_acc[((size_t)l * B + g) * PW + 4 * v];
         atomicAdd(dst, (double)acc.x);
@@ -345,7 +415,13 @@ gin_pool_kernel(int L, const int32_t* __restrict__ node_off_v, int B, const int3
       for (int k = 0; k < per; ++k) {
         const int g = gid[rb + k];
         if (g < 0) break;
-        const float4 x = *reinterpret_cast<const float4*>(src + (size_t)(row0 + rb + k) * W + 4 * v);
+        const size_t e = (size_t)(row0 + rb + k) * W + 4 * v;
+        float4 x = *reinterpret_cast<const float4*>(src + e);
+        if (xf) {
+          x = make_float4(bn_tail_h(x.x, sca[0], sha[0], scb[0], shb[0]), bn_tail_h(x.y, sca[1], sha[1], scb[1], shb[1]),
+                          bn_tail_h(x.z, sca[2], sha[2], scb[2], shb[2]), bn_tail_h(x.w, sca[3], sha[3], scb[3], shb[3]));
+          *reinterpret_cast<float4*>(tail.h_out + e) = x;
+        }
         if (g != g_run) {
           flush(g_run);
           acc = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -506,6 +582,7 @@ static int run_forward(const FwdArgs& a) {
   GCCB_LAUNCH(gin_build_x0_kernel, grid, 256, 0, a.stream, d, node_off_v, B, pos_v, sub_deg, graph_id,
               a.params + a.lay.emb, x0);
   const float* hin = x0;
+  BnTailArgs below{};                 // BatchNorm tail of layer l-1, applied by the kernel that reads its output
   for (int l = 0; l < d.L - 1; ++l) {
     float* a_l = (float*)(a.acts + a.al.a[l]);
     float* z1 = (float*)(a.acts + a.al.z1[l]);
@@ -519,17 +596,18 @@ static int run_forward(const FwdArgs& a) {
     float* runb = a.running ? a.running + (size_t)(l * 3 + 2) * 2 * H : nullptr;
     const float* P = a.params;
     if (l == 0) {
-      auto k = gin_agg_gemm1_kernel<GCCB_DINP, H>;
+      auto k = gin_agg_gemm1_kernel<GCCB_DINP, H, false>;
       size_t sm = smem_gemm<GCCB_DINP, H>();
       gccb::ensure_dyn_smem(k, sm);
       GCCB_LAUNCH(k, grid, 256, sm, a.stream, node_off_v, B, indptr, indices, hin, P + a.lay.w1[l], d.din,
-                  P + a.lay.b1[l], 0.0f, a_l, z1, s1);
+                  P + a.lay.b1[l], 0.0f, a_l, z1, s1, BnTailArgs{});
     } else {
-      auto k = gin_agg_gemm1_kernel<H, H>;
-      size_t sm = smem_gemm<H, H>();
+      // hin = z2 of layer l-1; its BatchNorm tail (below) is applied on the gather, h[l-1] written on the way
+      auto k = gin_agg_gemm1_kernel<H, H, true>;
+      size_t sm = smem_gemm<H, H>() + 4 * H * sizeof(float);
       gccb::ensure_dyn_smem(k, sm);
       GCCB_LAUNCH(k, grid, 256, sm, a.stream, node_off_v, B, indptr, indices, hin, P + a.lay.w1[l], H,
-                  P + a.lay.b1[l], 0.0f, a_l, z1, s1);
+                  P + a.lay.b1[l], 0.0f, a_l, z1, s1, below);
     }
     {
       auto k = gin_bn_gemm2_kernel<H>;
@@ -542,16 +620,15 @@ static int run_forward(const FwdArgs& a) {
     GCCB_LAUNCH(kt, grid, 256, 0, a.stream, 0, node_off_v, B, z2, sa, P + a.lay.bna_w[l], P + a.lay.bna_b[l],
                 runa, sb, P + a.lay.bnb_w[l], P + a.lay.bnb_b[l], runb, d.bn_eps, use_running, upd,
                 d.bn_mom, sb, hout);
-    GCCB_LAUNCH(kt, grid, 256, 0, a.stream, 1, node_off_v, B, z2, sa, P + a.lay.bna_w[l], P + a.lay.bna_b[l],
-                runa, sb, P + a.lay.bnb_w[l], P + a.lay.bnb_b[l], runb, d.bn_eps, use_running, upd,
-                d.bn_mom, sb, hout);
-    hin = hout;
+    below = BnTailArgs{sa, P + a.lay.bna_w[l], P + a.lay.bna_b[l], runa, sb, P + a.lay.bnb_w[l], P + a.lay.bnb_b[l],
+                       runb, d.bn_eps, d.bn_mom, use_running, upd, hout};
+    hin = z2;
   }
   const uint32_t keep = (uint32_t)fmin((1.0 - (double)d.drop_p) * 4294967296.0, 4294967295.0);
   double* pool_acc = (double*)(a.acts + a.al.pool_acc);
   auto kpl = gin_pool_kernel<H>;
   GCCB_LAUNCH(kpl, grid, 256, 0, a.stream, d.L, node_off_v, B, graph_id, (const float*)x0, a.d_hptrs, a.al.PW,
-              pool_acc);
+              pool_acc, hin, below);
   auto kp = gin_pool_predict_kernel<H>;
   GCCB_LAUNCH(kp, (B + GCCB_GPB - 1) / GCCB_GPB, 256, 0, a.stream, d, node_off_v, B, (const double*)pool_acc, a.params, a.d_offs, a.d_offs + 8,
               a.al.PW, a.drop_key, a.drop_step, a.drop_base, keep, (float*)(a.acts + a.al.pooled),
@@ -764,7 +841,7 @@ static int run_forward_tc(const FwdArgs& a) {
   double* pool_acc = (double*)(a.acts + a.al.pool_acc);
   auto kpl = gin_pool_kernel<H>;
   GCCB_LAUNCH(kpl, grid, 256, 0, a.stream, d.L, node_off_v, B, graph_id, (const float*)x0, a.d_hptrs, a.al.PW,
-              pool_acc);
+              pool_acc, (const float*)nullptr, BnTailArgs{});
   auto kp = gin_pool_predict_kernel<H>;
   GCCB_LAUNCH(kp, (B + GCCB_GPB - 1) / GCCB_GPB, 256, 0, a.stream, d, node_off_v, B, (const double*)pool_acc, a.params, a.d_offs, a.d_offs + 8,
               a.al.PW, a.drop_key, a.drop_step, a.drop_base, keep, (float*)(a.acts + a.al.pooled),

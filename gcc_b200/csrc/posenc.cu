@@ -2165,7 +2165,7 @@ extern "C" int gccb_posenc(const gccb_batch_t* batch, int32_t pos_dim, int32_t n
 #ifndef GCCB_EMU
   // per caller stream: batches in flight do not serialise.  The size-class kernels are long-lived and go to
   // lowest-priority streams whatever the caller's priority (a caller may run its short sampler kernels high)
-  StreamKit* kit = stream_kit((cudaStream_t)stream, 0, true);
+  StreamKit* kit = stream_kit((cudaStream_t)stream, 0, SidePriority::kLowest);
   cudaStream_t* side = kit->side;
   cudaEvent_t ev_fork = kit->ev[5];
   cudaEvent_t* ev_join = kit->ev;
