@@ -9,17 +9,19 @@ import numpy as np
 from gcc_b200 import _capi
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-_lib = None
+_libs = {}
 
 
-def lib():
-    global _lib
-    if _lib is None:
+def lib(production_hub_deg=False):
+    """The emulated library.  production_hub_deg: the build with the product's hub threshold (GCCB_HUB_DEG = 256)
+    instead of the tests' 3, for the warp gathers of rows with up to 256 neighbours."""
+    if production_hub_deg not in _libs:
         spec = importlib.util.spec_from_file_location("build_emu", os.path.join(HERE, "emu", "build_emu.py"))
         mod = importlib.util.module_from_spec(spec)
         spec.loader.exec_module(mod)
-        _lib = _capi.bind(C.CDLL(mod.build()), require_all=False)
-    return _lib
+        path = mod.build(hub_deg=None) if production_hub_deg else mod.build()
+        _libs[production_hub_deg] = _capi.bind(C.CDLL(path), require_all=False)
+    return _libs[production_hub_deg]
 
 
 def ptr(a):

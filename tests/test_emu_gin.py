@@ -65,11 +65,18 @@ def _oracle_view(b, views, pos, v):
 def test_gin_forward_backward_vs_oracle(L, H, B_, hops):
     """(the third case spans several 64-row tiles: graphs straddle tile boundaries in the pooling,
     aggregation and weight-gradient kernels)"""
-    Lb = lib()
     rng = np.random.default_rng(L * 100 + H)
     b, views, pos = _batch(B_, hops)
     assert B_ < 10 or int(b.node_off[0, b.B]) > 128
     print("N =", int(b.node_off[0, b.B]))
+    _forward_backward_vs_oracle(lib(), L, H, b, views, pos, rng)
+
+
+def _forward_backward_vs_oracle(Lb, L, H, b, views, pos, rng, kink_flips=0):
+    """Both views through gccb_gin_forward / gccb_gin_backward (train mode, dropout on view 0) against the float64
+    oracle and its autograd gradients; the running statistics are updated by both forwards.  Gradients: every entry
+    within rtol 2e-3 + 2e-4 of the tensor's scale, except at most `kink_flips` entries per tensor, which must still be
+    within 5e-3 of the scale (a ReLU pre-activation within fp32 noise of zero lands on the other side of the kink)."""
     cfg = glayout.make_cfg(num_layers=L, hidden=H)
     lay = glayout.c_layout(Lb, cfg)
     flat, sd, sl = _params(cfg, rng)
@@ -121,10 +128,52 @@ def test_gin_forward_backward_vs_oracle(L, H, B_, hops):
                 # bias feeding a train-mode BatchNorm: the true gradient is exactly 0; fp32 gives noise
                 assert np.abs(got).max() < 1e-5, (view, k_, np.abs(got).max())
                 continue
-            assert np.allclose(got, want, rtol=2e-3, atol=2e-4 * scale), (view, k_, np.abs(got - want).max(), scale)
+            bad = ~np.isclose(got, want, rtol=2e-3, atol=2e-4 * scale)
+            assert bad.sum() <= kink_flips and np.abs(got - want).max() <= 5e-3 * scale, \
+                (view, k_, int(bad.sum()), np.abs(got - want).max(), scale)
     # running statistics: both forwards updated the same buffers (two train-mode passes)
     assert np.all(nbt == 2)
     assert not np.allclose(running, running0)
+
+
+def _spread_degree_batch():
+    """Two ego-nets (the same in both views, in swapped order) whose rows have every degree residue mod 8 between 4
+    and 300: centre i is joined to leaves 0 .. d_i - 1 of a shared leaf pool, d_i = 4 .. 19, 250 .. 257 and 300, so
+    leaf j has degree #{i : d_i > j} and the pool spans the degrees in between."""
+    def net(ds, extra):
+        n_c, n_l = len(ds), max(ds) + extra
+        src = np.concatenate([np.full(d, i) for i, d in enumerate(ds)])
+        dst = n_c + np.concatenate([np.arange(d) for d in ds])
+        src, dst = np.concatenate([src, dst]), np.concatenate([dst, src])
+        order = np.lexsort((dst, src))
+        n = n_c + n_l
+        indptr = np.concatenate([[0], np.cumsum(np.bincount(src, minlength=n))])
+        return dict(subv=np.arange(n), indptr=indptr, indices=dst[order], n=n, m=len(src))
+    g0 = net(list(range(4, 20)) + list(range(250, 258)) + [300], 3)
+    g1 = net([5, 13, 21, 29, 37, 45, 53, 61, 120, 201], 2)
+    views = [[g0, g1], [g1, g0]]
+    b = NpBatch.from_subgraphs(views)
+    pos = np.random.default_rng(8).normal(0, 0.3, (2, b.node_cap, 32)).astype(np.float32)
+    return b, views, pos
+
+
+@pytest.mark.parametrize("L,H", [(3, 32), (3, 64), (3, 128)])
+def test_gin_warp_gathers_at_production_hub_threshold(L, H):
+    """The emulated kernels built with the product's hub threshold (GCCB_HUB_DEG = 256) instead of the tests' 3: rows
+    with 4..256 neighbours take the warp gathers (gather_range: eight neighbours per step, then the remainder;
+    gather_range4: four, then the remainder), in the forward aggregation and in the backward's dh gathers, and
+    every residue of the degree mod 8 occurs; rows with more neighbours still take the CTA-wide hub path."""
+    b, views, pos = _spread_degree_batch()
+    for v in (0, 1):
+        N = int(b.node_off[v, b.B])
+        deg = np.diff(b.indptr[v, :N + 1])
+        warp = deg[(deg >= 4) & (deg <= 256)]
+        assert set(warp % 8) == set(range(8)) and (deg > 256).sum() == 2 and deg.min() <= 3
+    # Rows that sum 250..300 neighbours put a few ReLU pre-activations within fp32 noise of zero: with (L, H) = (3, 64)
+    # one to four entries of a tensor land on the other side of a kink and differ from the oracle by up to 2.3e-3
+    # of the tensor's scale (the warp and hub gathers agree with each other to 5e-6 relative), hence kink_flips
+    _forward_backward_vs_oracle(lib(production_hub_deg=True), L, H, b, views, pos, np.random.default_rng(L * 10 + H),
+                                kink_flips=4)
 
 
 def test_stash_layout_locates_the_forward_intermediates(monkeypatch):
