@@ -93,6 +93,16 @@ _PROTOS = {
     "gccb_tc_gemm_bf16": (C.c_int, [p, p, C.c_int32, C.c_int32, C.c_int32, p, p, C.c_float, p, p, C.c_int32, p,
                                     C.c_int32, p, p]),
     "gccb_cast_bf16": (C.c_int, [p, C.c_int32, C.c_int32, C.c_int32, p, C.c_int32, C.c_int32, C.c_int32, p, p]),
+    "gccb_spmm_f64": (C.c_int, [p, p, p, C.c_int64, C.c_int32, C.c_int64, C.c_double, C.c_double, p, p, C.c_double,
+                                p, C.c_double, p, p, p]),
+    "gccb_graphwave_workspace": (C.c_size_t, [C.c_int64, C.c_int32]),
+    "gccb_graphwave": (C.c_int, [p, p, p, C.c_int64, p, C.c_int32, p, C.c_int32, C.c_int32, p, C.c_size_t, p, p]),
+    "gccb_prone_factor_workspace": (C.c_size_t, [C.c_int64]),
+    "gccb_prone_factor": (C.c_int, [p, p, p, C.c_int64, p, C.c_size_t, p, p, p]),
+    "gccb_gaussian_f64": (C.c_int, [p, C.c_int64, C.c_int32, C.c_uint64, p]),
+    "gccb_prone_propagate_workspace": (C.c_size_t, [C.c_int64, C.c_int32]),
+    "gccb_prone_propagate": (C.c_int, [p, p, p, C.c_int64, p, C.c_int32, C.c_double, p, C.c_int32, p, C.c_size_t,
+                                       p, p]),
 }
 
 SYMBOLS = tuple(_PROTOS)

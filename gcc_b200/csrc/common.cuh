@@ -78,6 +78,7 @@ inline void ensure_dyn_smem(K kern, size_t bytes) {
 #define GCCB_TAG_WALK 0u
 #define GCCB_TAG_SEED 1u
 #define GCCB_TAG_DROPOUT 2u
+#define GCCB_TAG_PRONE 3u
 
 // device status flag bits (gccb200.h: GCCB_FLAG_*)
 namespace gccb {

@@ -60,8 +60,10 @@ class FromNumpyAlign:
 
 def _baseline(name):
     def make(*args, **kwargs):
-        raise NotImplementedError("the %s baseline is not part of this project; evaluate embeddings saved by "
-                                  "generate.py with --model from_numpy / from_numpy_graph / from_numpy_align" % name)
+        raise NotImplementedError("the %s baseline is not a build_model model; save its rows with `python -m "
+                                  "gcc_b200.tasks.baselines --model %s ...` (or embeddings saved by generate.py) and "
+                                  "evaluate them with --model from_numpy / from_numpy_graph / from_numpy_align"
+                                  % (name, name.lower()))
     return make
 
 

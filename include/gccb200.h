@@ -317,6 +317,44 @@ int gccb_tc_gemm_bf16(const void* A, const void* B, int32_t M_cap, int32_t N, in
 int gccb_cast_bf16(const float* src, int32_t rows, int32_t cols, int32_t lds, void* dst, int32_t rows_pad,
                    int32_t cols_pad, int32_t transpose, const int32_t* rows_dev, gccb_stream_t stream);
 
+/* ---- embedding baselines in float64 (csrc/baselines.cu) -------------------------------------------
+ * GraphWave (gcc/models/emb/_graphwave) and ProNE (gcc/models/emb/prone.py) for the frozen-embedding
+ * tasks.  A graph is a symmetric CSR: indptr [n+1], indices [nnz] ascending per row, and vals [nnz]
+ * (NULL: each entry weighs 1, a repeated column being a parallel edge).  Dense blocks are n x k
+ * row-major with row stride ld.  Blocks whose rows all start on 16 bytes (16-byte aligned base pointers and
+ * an even ld) take the 128-bit path, any other layout the 64-bit one; the results are the same.
+ *
+ * Y = alpha * dr * ((A + sigma I) (dc X)) + beta X + gamma Z; dr, dc, Z may be NULL (1, 1, no term).
+ * Y may alias Z, not X.                                                                                */
+int gccb_spmm_f64(const int64_t* indptr, const int32_t* indices, const double* vals, int64_t n, int32_t k,
+                  int64_t ld, double alpha, double sigma, const double* dr, const double* dc, double beta,
+                  const double* X, double gamma, const double* Z, double* Y, gccb_stream_t stream);
+/* GraphWave's chi [n][4 n_times]: row u holds, per scale s and time point t, (1/n) sum_i cos and sin of
+ * times[t] * heat_s[i,u], heat_s = sum_k cheb[s*(order+1)+k] T_k(L - I) with L the normalised Laplacian and
+ * entries <= 1e-4/n set to 0.  cheb (host, [2][order+1]) and times (host, [n_times <= 64]) come from the
+ * caller.  The heat is built bc identity columns at a time in a workspace of
+ * gccb_graphwave_workspace(n, bc) bytes and never held whole; the result does not depend on bc.       */
+size_t gccb_graphwave_workspace(int64_t n, int32_t bc);
+int gccb_graphwave(const int64_t* indptr, const int32_t* indices, const double* vals, int64_t n,
+                   const double* cheb, int32_t order, const double* times, int32_t n_times, int32_t bc,
+                   void* workspace, size_t workspace_bytes, double* chi, gccb_stream_t stream);
+/* ProNE's sparse factorization on A's pattern: F[e] = log(A_ij / d_i) - log(A_ij neg_j) for entry e =
+ * (i, j), d the row sums, neg_j = (sum_i A_ij / d_i)^0.75 normalised to sum 1; FT[e] = F_ji, the entries
+ * of F^T on the same (symmetric) pattern.                                                            */
+size_t gccb_prone_factor_workspace(int64_t n);
+int gccb_prone_factor(const int64_t* indptr, const int32_t* indices, const double* vals, int64_t n,
+                      void* workspace, size_t workspace_bytes, double* F, double* FT, gccb_stream_t stream);
+/* out [rows][cols]: standard normals by Box-Muller on Philox counters (row, col, 0, GCCB_TAG_PRONE),
+ * key = run seed: the start block of ProNE's randomized SVD.                                         */
+int gccb_gaussian_f64(double* out, int64_t rows, int32_t cols, uint64_t key, gccb_stream_t stream);
+/* ProNE's spectral propagation of a [n][k] (order >= 2, bessel (host) = I_0 .. I_{order-1} at theta):
+ * M = (1 - mu) I - DA with DA = (I + A) row-l1-normalised, Chebyshev terms Lx_i, conv = sum of
+ * +-2 I_i Lx_i (I_0 a for i = 0), mm [n][k] = (I + A)(a - conv).                                     */
+size_t gccb_prone_propagate_workspace(int64_t n, int32_t k);
+int gccb_prone_propagate(const int64_t* indptr, const int32_t* indices, const double* vals, int64_t n,
+                         const double* a, int32_t k, double mu, const double* bessel, int32_t order,
+                         void* workspace, size_t workspace_bytes, double* mm, gccb_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
