@@ -53,6 +53,23 @@ class GinStash(C.Structure):
                 [(n, C.c_int32) for n in ("cap_pad", "splits", "DW", "PW")])
 
 
+class GatCfg(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("num_layers", "hidden", "num_heads", "pos_dim", "deg_dim", "max_degree",
+                                         "set2set_iter", "set2set_layers", "norm")] + [("norm_eps", C.c_float)]
+
+
+class GatLayout(C.Structure):
+    _fields_ = ([(n, C.c_int64 * 8) for n in ("fc", "attn_l", "attn_r")] + [("emb", C.c_int64)] +
+                [(n, C.c_int64 * 8) for n in ("w_ih", "w_hh", "b_ih", "b_hh")] +
+                [(n, C.c_int64) for n in ("ro0_w", "ro0_b", "ro2_w", "ro2_b", "total")])
+
+
+class GatStash(C.Structure):
+    _fields_ = ([("x0", C.c_int64)] + [(n, C.c_int64 * 8) for n in ("z", "h", "att")] +
+                [(n, C.c_int64) for n in ("qstar", "hs", "cs", "gates", "alpha", "y1", "score",
+                                          "dh", "dz", "dout", "sv", "dx0", "dgates", "dy")])
+
+
 _PROTOS = {
     "gccb_version": (C.c_int, []),
     "gccb_arch": (C.c_int, []),
@@ -73,6 +90,12 @@ _PROTOS = {
     "gccb_gin_backward": (C.c_int, [C.POINTER(GinCfg), C.POINTER(Batch), C.c_int32, p, p, p, p,
                                     C.c_uint64, C.c_uint64, C.c_int32, p, C.c_size_t, p]),
     "gccb_gin_stash_layout": (C.c_int, [C.POINTER(GinCfg), C.c_int32, C.c_int32, C.POINTER(GinStash)]),
+    "gccb_gat_param_layout": (C.c_int, [C.POINTER(GatCfg), C.POINTER(GatLayout)]),
+    "gccb_gat_acts_bytes": (C.c_size_t, [C.POINTER(GatCfg), C.c_int32, C.c_int32]),
+    "gccb_gat_forward": (C.c_int, [C.POINTER(GatCfg), C.POINTER(Batch), C.c_int32, p, p, p, C.c_size_t, p, p]),
+    "gccb_gat_backward_workspace": (C.c_size_t, [C.POINTER(GatCfg), C.c_int32, C.c_int32]),
+    "gccb_gat_backward": (C.c_int, [C.POINTER(GatCfg), C.POINTER(Batch), C.c_int32, p, p, p, p, p, C.c_size_t, p]),
+    "gccb_gat_stash_layout": (C.c_int, [C.POINTER(GatCfg), C.c_int32, C.c_int32, C.POINTER(GatStash)]),
     "gccb_moco_logits": (C.c_int, [p, p, p, C.c_int32, C.c_int32, C.c_int32, C.c_float, p, p]),
     "gccb_moco_logits_backward": (C.c_int, [p, p, p, C.c_int32, C.c_int32, C.c_int32, C.c_float,
                                             p, p]),

@@ -409,4 +409,21 @@ __device__ __forceinline__ void tile_colstats(const float (&v)[4][TileCols<NOUT>
   __syncthreads();
 }
 
+// Kernels of the GIN path that the GAT encoder (gat.cu) launches as they are: the input assembly, the split-K
+// weight gradient with its reduce, and the degree-embedding scatter.
+__global__ void __launch_bounds__(256)
+gin_build_x0_kernel(GinDims d, const int32_t* __restrict__ node_off_v, int B, const float* __restrict__ pos,
+                    const int32_t* __restrict__ sub_deg, const int32_t* __restrict__ graph_id,
+                    const float* __restrict__ emb, float* __restrict__ x0);
+__global__ void __launch_bounds__(256)
+gin_wgrad_kernel(const int32_t* __restrict__ node_off_v, int B, int H, int KQ, const float* __restrict__ P,
+                 const float* __restrict__ Q, const double* __restrict__ q_sums, const float* __restrict__ q_gamma,
+                 const float* __restrict__ q_beta, float bn_eps, float* __restrict__ part);
+__global__ void __launch_bounds__(256)
+gin_wgrad_reduce_kernel(int H, int KQ, int in_features, const float* __restrict__ part, float* __restrict__ gw,
+                        float* __restrict__ gb);
+__global__ void __launch_bounds__(256)
+gin_bwd_emb_kernel(GinDims d, const int32_t* __restrict__ node_off_v, int B, const int32_t* __restrict__ sub_deg,
+                   const float* __restrict__ dx0, float* __restrict__ gemb);
+
 }  // namespace gccb

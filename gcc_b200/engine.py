@@ -2,9 +2,9 @@
 feeds it) as a fixed sequence of libgccb200 kernel launches with no host synchronisation:
 
   draw seeds -> RWR walk / induce / batch -> positional features           (datasets/)
-  -> GIN forward q (model) and k (model_ema, BN in train mode, train.py:357-365)
+  -> encoder forward q (model) and k (model_ema, BN in train mode, train.py:357-365)
   -> fused InfoNCE (loss, dq; logits never materialised)                     (memory_moco.py, criterions.py)
-  -> GIN backward -> [all-gather of keys+grads when world > 1]
+  -> encoder backward -> [all-gather of keys+grads when world > 1]
   -> clip + optimiser step (Adam, SGD or Adagrad) + momentum update on flat buffers (train.py:409-417,430-431)
   -> FIFO enqueue of the keys (memory_moco.py:55-61)
 
@@ -81,15 +81,12 @@ class PretrainEngine:
         self.feat_k = self.xch.keys_send if self.xch else torch.zeros(B, H, **f32)
         self.dq = torch.zeros(B, H, **f32)
         self.dk = torch.zeros(B, H, **f32)
-        self.pooled = torch.zeros(max(L - 1, 1), B, H, **f32)
-        self.pooled_k = torch.zeros(max(L - 1, 1), B, H, **f32)
         self.aux_stream = self._new_stream(0, -1)      # key encoder, concurrent with the query encoder
         cap = dataset.node_cap
-        acts_bytes = self.lib.gccb_gin_acts_bytes(C.byref(model.cfg), B, cap)
+        acts_bytes = model.acts_bytes(B, cap)
         self.acts_q = torch.empty(acts_bytes, dtype=torch.uint8, device=dev)
         self.acts_k = torch.empty(acts_bytes, dtype=torch.uint8, device=dev)
-        self.bwd_ws = torch.empty(self.lib.gccb_gin_backward_workspace(C.byref(model.cfg), B, cap),
-                                  dtype=torch.uint8, device=dev)
+        self.bwd_ws = torch.empty(model.backward_workspace_bytes(B, cap), dtype=torch.uint8, device=dev)
         K = contrast.queueSize
         self.K = K
         self.nce_ws = torch.empty(max(self.lib.gccb_infonce_workspace(B, H, K), B * B * 4, 8),
@@ -238,10 +235,10 @@ class PretrainEngine:
             cur = torch.cuda.current_stream(self.dev)
             self.aux_stream.wait_stream(cur)
             with torch.cuda.stream(self.aux_stream):
-                ema._run_forward(gk, False, drop_step=0, drop_base=-1, acts=self.acts_k, feat=self.feat_k,
-                                 pooled=self.pooled_k, bn_train=True)
-        _, _, saved_q = model._run_forward(gq, True, drop_step=step, drop_base=0, acts=self.acts_q,
-                                           feat=self.feat_q, pooled=self.pooled, bn_train=True)
+                ema._run_forward(gk, False, step=step, dropout=False, acts=self.acts_k, feat=self.feat_k,
+                                 all_outputs=False, bn_train=True)
+        _, _, saved_q = model._run_forward(gq, True, step=step, dropout=True, acts=self.acts_q, feat=self.feat_q,
+                                           all_outputs=False, bn_train=True)
         self.grads.zero_()
         if self.moco:
             cur.wait_stream(self.aux_stream)
@@ -252,8 +249,8 @@ class PretrainEngine:
                        "gccb_infonce_fused")
             model._run_backward(gq, saved_q, self.dq, grads_flat=self.grads, ws=self.bwd_ws)
         else:
-            _, _, saved_k = model._run_forward(gk, True, drop_step=step, drop_base=L, acts=self.acts_k,
-                                               feat=self.feat_k, pooled=self.pooled, bn_train=True)
+            _, _, saved_k = model._run_forward(gk, True, step=step, dropout=True, acts=self.acts_k, feat=self.feat_k,
+                                               all_outputs=False, bn_train=True)
             _lib.check(lib.gccb_e2e_nce(_lib.dptr(self.feat_q), _lib.dptr(self.feat_k), b, H, self.T,
                                         _lib.dptr(self.stats), _lib.dptr(self.dq), _lib.dptr(self.dk),
                                         _lib.dptr(self.nce_ws), self.nce_ws.numel(), st), "gccb_e2e_nce")

@@ -1,6 +1,7 @@
 """GraphEncoder with the reference's constructor, forward signature and state_dict keys
-(gcc/models/graph_encoder.py:19-200, gin branch; SURVEY.md section 8b), executing as
-hand-written sm_90a kernels through libgccb200 (csrc/gin_fwd.cu, csrc/gin_bwd.cu).
+(gcc/models/graph_encoder.py:19-200, gin and gat branches; SURVEY.md section 8b), executing as
+hand-written sm_90a kernels through libgccb200 (csrc/gin_fwd.cu, csrc/gin_bwd.cu; csrc/gat.cu for gnn_model="gat",
+whose Set2Set and lin_readout are live parameters in the flat buffer).
 
 All live parameters are views into ONE flat fp32 buffer (models/layout.py) followed by the
 unused-but-present tensors of the reference module (set2set.*, lin_readout.*), so that
@@ -41,20 +42,21 @@ def _child(mod, name, cls=_Holder):
     return mod._modules[name]
 
 
-class _GinEncodeFn(torch.autograd.Function):
+class _EncodeFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, module, g, need_grad, *params):
-        # (grad mode is always off inside Function.forward; the caller decides)
+    def forward(ctx, module, g, need_grad, pooled_out, *params):
+        # (grad mode is always off inside Function.forward; the caller decides).  The GIN path's per-layer pooled
+        # outputs leave through pooled_out, outside the graph: they never receive a gradient
         feat, pooled, saved = module._run_forward(g, keep_for_backward=need_grad)
         ctx.module, ctx.g, ctx.saved = module, g, saved
-        ctx.mark_non_differentiable(pooled)
-        return feat, pooled
+        pooled_out.append(pooled)
+        return feat
 
     @staticmethod
-    def backward(ctx, dfeat, _dpooled):
+    def backward(ctx, dfeat):
         grads = ctx.module._run_backward(ctx.g, ctx.saved, dfeat.contiguous())
         ctx.saved = None
-        return (None, None, None) + tuple(grads)
+        return (None, None, None, None) + tuple(grads)
 
 
 class GraphEncoder(nn.Module):
@@ -64,20 +66,28 @@ class GraphEncoder(nn.Module):
                  num_layer_set2set=3, norm=False, gnn_model="mpnn", degree_input=False,
                  lstm_as_gate=False):
         super(GraphEncoder, self).__init__()
-        if gnn_model != "gin":
-            raise NotImplementedError("only gnn_model='gin' (train.py:77 default, the north-star path) "
-                                      "is implemented; mpnn/gat are out of scope (SURVEY.md section 2)")
+        if gnn_model == "mpnn":
+            raise NotImplementedError("gnn_model='mpnn' does not run in the reference either: GraphEncoder.forward "
+                                      "passes e_feat=None (graph_encoder.py:188) into NNConv's edge network")
+        if gnn_model not in ("gin", "gat"):
+            raise NotImplementedError("gnn_model must be 'gin' or 'gat', not %r" % (gnn_model,))
         if not degree_input:
             raise NotImplementedError("degree_input=False is never used by train.py (:618)")
         if output_dim != node_hidden_dim:
             raise NotImplementedError("output_dim must equal node_hidden_dim (train.py:612-613)")
         self.gnn_model, self.norm, self.degree_input = gnn_model, norm, degree_input
         self.max_node_freq, self.max_edge_freq, self.max_degree = max_node_freq, max_edge_freq, max_degree
+        self._scratch = {}
+        if gnn_model == "gat":
+            self._init_gat(positional_embedding_size, degree_embedding_size, max_degree, node_hidden_dim, num_layers,
+                           num_heads, num_step_set2set, num_layer_set2set, norm)
+            return
         H, L = node_hidden_dim, num_layers
         self.cfg = glayout.make_cfg(num_layers=L, hidden=H, pos_dim=positional_embedding_size,
                                     deg_dim=degree_embedding_size, max_degree=max_degree, norm=norm)
         self._slices, self._n_live = glayout.param_slices(self.cfg)
         self._rslices, self._n_run = glayout.running_slices(self.cfg)
+        self._nbt_keys = glayout.nbt_keys(self.cfg)
         din = positional_embedding_size + degree_embedding_size + 1
         # ---- draw initial values in the reference's construction order (gin.py:152-197,
         #      graph_encoder.py:92-130) so that a given torch seed yields the same weights
@@ -151,7 +161,56 @@ class GraphEncoder(nn.Module):
         self._bind_views(register=True)
         self.dropout_key = 0x9E3779B97F4A7C15 ^ (torch.initial_seed() & 0xFFFFFFFFFFFF)
         self._drop_step = 0
-        self._scratch = {}
+
+    def _init_gat(self, P, D, max_degree, H, L, nh, T, K, norm):
+        """gnn_model="gat": UnsupervisedGAT (gat.py), Set2Set(H, T, K) and lin_readout, every parameter live."""
+        if H % nh:
+            raise ValueError("node_hidden_dim %d is not a multiple of num_heads %d (gat.py:20)" % (H, nh))
+        self.cfg = glayout.make_gat_cfg(num_layers=L, hidden=H, num_heads=nh, pos_dim=P, deg_dim=D,
+                                        max_degree=max_degree, set2set_iter=T, set2set_layers=K, norm=norm)
+        self._slices, self._n_live = glayout.gat_param_slices(self.cfg)
+        self._rslices, self._n_run, self._nbt_keys = {}, 0, []
+        self._dead_slices, self._n_all = {}, self._n_live
+        din = P + D + 1
+        # ---- initial values in the reference's construction order: per layer GATConv's Linear(in, H, bias=False)
+        #      (its kaiming draw), then its reset_parameters (xavier_normal_, gain('relu'), on fc.weight, attn_l,
+        #      attn_r; the attention vectors are uninitialised before it); degree_embedding; Set2Set's LSTM, drawn
+        #      twice (its constructor, then dgl Set2Set's reset_parameters); lin_readout (graph_encoder.py:82-129)
+        init = {}
+        gain = nn.init.calculate_gain("relu")
+        for i in range(L):
+            p = "gnn.layers.%d.gnn." % i
+            fc = nn.Linear(din if i == 0 else H, H, bias=False)
+            attn_l, attn_r = torch.empty(1, nh, H // nh), torch.empty(1, nh, H // nh)
+            nn.init.xavier_normal_(fc.weight, gain=gain)
+            nn.init.xavier_normal_(attn_l, gain=gain)
+            nn.init.xavier_normal_(attn_r, gain=gain)
+            init[p + "fc.weight"], init[p + "attn_l"], init[p + "attn_r"] = fc.weight, attn_l, attn_r
+        init["degree_embedding.weight"] = nn.Embedding(max_degree + 1, D).weight
+        lstm = nn.LSTM(2 * H, H, K)
+        lstm.reset_parameters()              # dgl Set2Set.__init__ -> reset_parameters -> lstm.reset_parameters()
+        for n, p_ in lstm.named_parameters():
+            init["set2set.lstm." + n] = p_
+        ro0, ro2 = nn.Linear(2 * H, H), nn.Linear(H, H)
+        init["lin_readout.0.weight"], init["lin_readout.0.bias"] = ro0.weight, ro0.bias
+        init["lin_readout.2.weight"], init["lin_readout.2.bias"] = ro2.weight, ro2.bias
+        flat = torch.zeros(self._n_all)
+        for key, (o, shape) in self._slices.items():
+            flat[o:o + init[key].numel()] = init[key].detach().reshape(-1)
+        # ---- module tree with the reference's names
+        layers = _child(_child(self, "gnn"), "layers")
+        for i in range(L):
+            _child(_child(_child(layers, str(i)), "gnn"), "fc")
+        _child(self, "degree_embedding")
+        _child(_child(self, "set2set"), "lstm")
+        ro = _child(self, "lin_readout")
+        _child(ro, "0")
+        ro.add_module("1", nn.ReLU())
+        _child(ro, "2")
+        self._flat = flat
+        self._running = torch.zeros(0)
+        self._nbt = torch.zeros(0, dtype=torch.long)
+        self._bind_views(register=True)
 
     # ---------------------------------------------------------------------------------------------
     def _resolve(self, key):
@@ -184,7 +243,7 @@ class GraphEncoder(nn.Module):
                 mod.register_buffer(leaf, view)
             else:
                 mod._buffers[leaf] = view
-        for i, key in enumerate(glayout.nbt_keys(self.cfg)):
+        for i, key in enumerate(self._nbt_keys):
             mod, leaf = self._resolve(key)
             if register:
                 mod.register_buffer(leaf, self._nbt[i])
@@ -205,7 +264,7 @@ class GraphEncoder(nn.Module):
             mod, leaf = self._resolve(key)
             running[o:o + shape[0]] = mod._buffers[leaf].float()
         nbt = torch.empty(len(self._nbt), dtype=torch.long, device=dev)
-        for i, key in enumerate(glayout.nbt_keys(self.cfg)):
+        for i, key in enumerate(self._nbt_keys):
             mod, leaf = self._resolve(key)
             nbt[i] = mod._buffers[leaf]
         self._flat, self._running, self._nbt = flat, running, nbt
@@ -231,9 +290,18 @@ class GraphEncoder(nn.Module):
         return self.gnn.batch_norms._modules["0"].training
 
     # ---------------------------------------------------------------------------------------------
+    def acts_bytes(self, batch, node_cap):
+        """Bytes of the activation stash one forward of a batch leaves for its backward."""
+        fn = _lib.get().gccb_gat_acts_bytes if self.gnn_model == "gat" else _lib.get().gccb_gin_acts_bytes
+        return fn(C.byref(self.cfg), batch, node_cap)
+
+    def backward_workspace_bytes(self, batch, node_cap):
+        fn = (_lib.get().gccb_gat_backward_workspace if self.gnn_model == "gat"
+              else _lib.get().gccb_gin_backward_workspace)
+        return fn(C.byref(self.cfg), batch, node_cap)
+
     def _acts_buffer(self, g, fresh):
-        lib = _lib.get()
-        nbytes = lib.gccb_gin_acts_bytes(C.byref(self.cfg), g.buffers.B, g.buffers.node_cap)
+        nbytes = self.acts_bytes(g.buffers.B, g.buffers.node_cap)
         if fresh:
             return torch.empty(nbytes, dtype=torch.uint8, device=self._flat.device)
         key = ("acts", nbytes)
@@ -241,19 +309,38 @@ class GraphEncoder(nn.Module):
             self._scratch[key] = torch.empty(nbytes, dtype=torch.uint8, device=self._flat.device)
         return self._scratch[key]
 
-    def _run_forward(self, g, keep_for_backward, drop_step=None, drop_base=None, acts=None, feat=None,
-                     pooled=None, bn_train=None):
-        lib = _lib.get()
+    def _run_forward(self, g, keep_for_backward, step=None, dropout=None, acts=None, feat=None, all_outputs=True,
+                     bn_train=None):
+        """One view through the encoder's kernels.  The engine passes step (its step index), dropout (whether the
+        view's dropout masks are drawn), bn_train, and its own acts / feat buffers; the module-level forward passes
+        none of them.  all_outputs=False skips the per-layer pooled outputs.  Returns (feat, all outputs or None,
+        what _run_backward needs)."""
         buf = g.buffers
         dev = self._flat.device
-        B, H, L = buf.B, self.cfg.hidden, self.cfg.num_layers
+        B, H = buf.B, self.cfg.hidden
         if acts is None:
             acts = self._acts_buffer(g, fresh=keep_for_backward)
         if feat is None:
             feat = torch.empty(B, H, dtype=torch.float32, device=dev)
-        if pooled is None:
-            pooled = torch.empty(L - 1, B, H, dtype=torch.float32, device=dev)
-        if drop_base is None:
+        if self.gnn_model == "gat":
+            rc = _lib.get().gccb_gat_forward(C.byref(self.cfg), C.byref(buf.c), g.view, _lib.dptr(buf.pos),
+                                             _lib.dptr(self._flat), _lib.dptr(acts), acts.numel(), _lib.dptr(feat),
+                                             _lib.stream_ptr())
+            _lib.check(rc, "gccb_gat_forward")
+            return feat, None, acts
+        return self._run_gin_forward(g, acts, feat, step, dropout, all_outputs, bn_train)
+
+    def _run_gin_forward(self, g, acts, feat, step, dropout, all_outputs, bn_train):
+        lib = _lib.get()
+        buf = g.buffers
+        dev = self._flat.device
+        B, H, L = buf.B, self.cfg.hidden, self.cfg.num_layers
+        pooled = torch.empty(L - 1, B, H, dtype=torch.float32, device=dev) if all_outputs else None
+        drop_step = drop_base = None
+        if dropout is not None:
+            # mask layer ids: q view 0..L-1, k view L..2L-1; no dropout = eval dropout
+            drop_base, drop_step = (g.view * L, step) if dropout else (-1, 0)
+        else:
             if self.gnn.drop.training:
                 # mask layer ids: q view 0..L-1, k view L..2L-1 (E2E runs both views through this
                 # module); the step index advances with every q-view forward
@@ -276,7 +363,6 @@ class GraphEncoder(nn.Module):
 
     def _run_backward(self, g, saved, dfeat, grads_flat=None, ws=None):
         lib = _lib.get()
-        acts, drop_step, drop_base = saved
         buf = g.buffers
         dev = self._flat.device
         own = grads_flat is None
@@ -285,15 +371,22 @@ class GraphEncoder(nn.Module):
             # them), so a buffer must never be recycled by a later backward
             grads_flat = torch.zeros(self._n_live, dtype=torch.float32, device=dev)
         if ws is None:
-            nbytes = lib.gccb_gin_backward_workspace(C.byref(self.cfg), buf.B, buf.node_cap)
+            nbytes = self.backward_workspace_bytes(buf.B, buf.node_cap)
             key = ("bwd", nbytes)
             if key not in self._scratch:
                 self._scratch[key] = torch.empty(nbytes, dtype=torch.uint8, device=dev)
             ws = self._scratch[key]
-        rc = lib.gccb_gin_backward(C.byref(self.cfg), C.byref(buf.c), g.view, _lib.dptr(self._flat),
-                                   _lib.dptr(acts), _lib.dptr(dfeat), _lib.dptr(grads_flat), self.dropout_key,
-                                   drop_step, drop_base, _lib.dptr(ws), ws.numel(), _lib.stream_ptr())
-        _lib.check(rc, "gccb_gin_backward")
+        if self.gnn_model == "gat":
+            rc = lib.gccb_gat_backward(C.byref(self.cfg), C.byref(buf.c), g.view, _lib.dptr(self._flat),
+                                       _lib.dptr(saved), _lib.dptr(dfeat), _lib.dptr(grads_flat), _lib.dptr(ws),
+                                       ws.numel(), _lib.stream_ptr())
+            _lib.check(rc, "gccb_gat_backward")
+        else:
+            acts, drop_step, drop_base = saved
+            rc = lib.gccb_gin_backward(C.byref(self.cfg), C.byref(buf.c), g.view, _lib.dptr(self._flat),
+                                       _lib.dptr(acts), _lib.dptr(dfeat), _lib.dptr(grads_flat), self.dropout_key,
+                                       drop_step, drop_base, _lib.dptr(ws), ws.numel(), _lib.stream_ptr())
+            _lib.check(rc, "gccb_gin_backward")
         if not own:
             return None
         out = []
@@ -306,10 +399,12 @@ class GraphEncoder(nn.Module):
 
     def forward(self, g, return_all_outputs=False):
         """g: gcc_b200.datasets.BatchedSubgraphs (the batched DGLGraph stand-in).
-        Returns Tensor[B, output_dim] or (x, [L-1 x Tensor[B, hidden]]) (graph_encoder.py:197-200)."""
+        Returns Tensor[B, output_dim] or (x, all_outputs) (graph_encoder.py:197-200): [L-1 x Tensor[B, hidden]] for
+        gin, None for gat."""
         _lib.require_device()
         need_grad = torch.is_grad_enabled() and any(p.requires_grad for p in self._live_params)
-        x, pooled = _GinEncodeFn.apply(self, g, need_grad, *self._live_params)
+        pooled = []
+        x = _EncodeFn.apply(self, g, need_grad, pooled, *self._live_params)
         if return_all_outputs:
-            return x, [pooled[i] for i in range(pooled.shape[0])]
+            return x, None if pooled[0] is None else [pooled[0][i] for i in range(pooled[0].shape[0])]
         return x

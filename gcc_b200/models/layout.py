@@ -91,3 +91,54 @@ def c_layout(lib, cfg):
     if rc:
         raise ValueError(lib.gccb_last_error().decode())
     return lay
+
+
+# ---- GAT encoder (gnn_model="gat"; include/gccb200.h: gccb_gat_layout_t) --------------------------------------
+def make_gat_cfg(num_layers=5, hidden=64, num_heads=4, pos_dim=32, deg_dim=16, max_degree=512, set2set_iter=6,
+                 set2set_layers=3, norm=True, norm_eps=1e-5):
+    return _capi.GatCfg(num_layers, hidden, num_heads, pos_dim, deg_dim, max_degree, set2set_iter, set2set_layers,
+                        int(bool(norm)), norm_eps)
+
+
+def gat_param_slices(cfg):
+    """OrderedDict key -> (offset, shape) of every GAT-encoder parameter, in flat-buffer order.  Pure-Python mirror
+    of gat_param_layout() in csrc/gat.cu (tests compare the two through gccb_gat_param_layout).  Keys are the
+    reference's: gnn.layers.{i}.gnn.* (dgl GATLayer wrapping GATConv), degree_embedding, set2set.lstm.*,
+    lin_readout.{0,2}.*."""
+    L, H, nh = cfg.num_layers, cfg.hidden, cfg.num_heads
+    din = cfg.pos_dim + cfg.deg_dim + 1
+    out = OrderedDict()
+    off = 0
+
+    def take(key, shape):
+        nonlocal off
+        n = 1
+        for s in shape:
+            n *= s
+        out[key] = (off, tuple(shape))
+        off += n
+
+    for i in range(L):
+        p = "gnn.layers.%d.gnn." % i
+        take(p + "fc.weight", (H, din if i == 0 else H))
+        take(p + "attn_l", (1, nh, H // nh))
+        take(p + "attn_r", (1, nh, H // nh))
+    take("degree_embedding.weight", (cfg.max_degree + 1, cfg.deg_dim))
+    for k in range(cfg.set2set_layers):
+        take("set2set.lstm.weight_ih_l%d" % k, (4 * H, 2 * H if k == 0 else H))
+        take("set2set.lstm.weight_hh_l%d" % k, (4 * H, H))
+        take("set2set.lstm.bias_ih_l%d" % k, (4 * H,))
+        take("set2set.lstm.bias_hh_l%d" % k, (4 * H,))
+    take("lin_readout.0.weight", (H, 2 * H))
+    take("lin_readout.0.bias", (H,))
+    take("lin_readout.2.weight", (H, H))
+    take("lin_readout.2.bias", (H,))
+    return out, off
+
+
+def gat_c_layout(lib, cfg):
+    lay = _capi.GatLayout()
+    rc = lib.gccb_gat_param_layout(C.byref(cfg), C.byref(lay))
+    if rc:
+        raise ValueError(lib.gccb_last_error().decode())
+    return lay

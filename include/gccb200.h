@@ -226,6 +226,68 @@ typedef struct {
 int gccb_gin_stash_layout(const gccb_gin_cfg_t* cfg, int32_t batch, int32_t node_cap,
                           gccb_gin_stash_t* out /* host */);
 
+/* ---- GAT encoder (--model gat) ----------------------------------------------------------
+ * Replaces GraphEncoder.forward with gnn_model="gat" (graph_encoder.py:132-200): UnsupervisedGAT
+ * (gat.py: num_layers DGL GATLayers, flatten, leaky_relu(0.01) between layers), dgl Set2Set and
+ * lin_readout, fp32.  The input X0 is the GIN path's.  Semantics as restated in DESIGN.md (GAT section).
+ * Every graph of the batch must be symmetric: the in-edges of v are row v of the batch CSR, and the
+ * backward reads the out-edges of u from row u.                                                       */
+typedef struct {
+  int32_t num_layers;      /* GAT layers, 1..8                        train.py --num-layer         */
+  int32_t hidden;          /* H = output_dim, 32 / 64 / 128 / 256                                  */
+  int32_t num_heads;       /* 1..8, H % num_heads == 0 (gat.py:20)                                 */
+  int32_t pos_dim;         /* as gccb_gin_cfg_t                                                    */
+  int32_t deg_dim;
+  int32_t max_degree;
+  int32_t set2set_iter;    /* Set2Set n_iters >= 1                    --set2set-iter               */
+  int32_t set2set_layers;  /* LSTM layers 1..8                        --set2set-lstm-layer         */
+  int32_t norm;            /* F.normalize on the output                                            */
+  float norm_eps;          /* 1e-5                                                                 */
+} gccb_gat_cfg_t;
+
+/* offsets (in floats) into the flat parameter buffer, in this order: per layer fc.weight [H][in],
+ * attn_l [nh][F], attn_r; degree_embedding; per LSTM layer weight_ih [4H][in], weight_hh [4H][H],
+ * bias_ih [4H], bias_hh [4H] (gate order i, f, g, o); lin_readout.0 weight [H][2H], bias; .2 weight
+ * [H][H], bias.  Unused entries are -1.                                                              */
+typedef struct {
+  int64_t fc[8], attn_l[8], attn_r[8];
+  int64_t emb;
+  int64_t w_ih[8], w_hh[8], b_ih[8], b_hh[8];
+  int64_t ro0_w, ro0_b, ro2_w, ro2_b;
+  int64_t total;           /* number of floats, all live */
+} gccb_gat_layout_t;
+int gccb_gat_param_layout(const gccb_gat_cfg_t* cfg, gccb_gat_layout_t* out /* host */);
+
+/* bytes of the activation stash one forward needs for its backward */
+size_t gccb_gat_acts_bytes(const gccb_gat_cfg_t* cfg, int32_t batch, int32_t node_cap);
+/* forward of ONE view; feat: [B][hidden].  No running state, no dropout.                            */
+int gccb_gat_forward(const gccb_gat_cfg_t* cfg, const gccb_batch_t* batch, int32_t view, const float* pos,
+                     const float* params, void* acts, size_t acts_bytes, float* feat, gccb_stream_t stream);
+/* backward of ONE view: grads += d loss / d params (flat, same layout; caller zeroes before the first
+ * view).  acts: the stash of the forward of the same view and parameters.                            */
+size_t gccb_gat_backward_workspace(const gccb_gat_cfg_t* cfg, int32_t batch, int32_t node_cap);
+int gccb_gat_backward(const gccb_gat_cfg_t* cfg, const gccb_batch_t* batch, int32_t view, const float* params,
+                      const void* acts, const float* dfeat, float* grads, void* workspace, size_t workspace_bytes,
+                      gccb_stream_t stream);
+
+/* Where the intermediates live (host-only query).  Forward, byte offsets into the stash: x0 float
+ * [node_cap][64]; z[l], h[l] float [node_cap][hidden] (h = the layer's output after its activation);
+ * att[l] float [4][node_cap][nh]: el | er | max | denominator of the edge softmax of each (row, head);
+ * qstar float [T+1][B][2H] (q* before each iteration, [0] = 0); hs, cs float [T+1][K][B][H] (LSTM h and c
+ * after each iteration, [0] = 0); gates float [T][K][B][4H] (i, f, g, o after their activations); alpha
+ * float [T][node_cap] (Set2Set attention); y1 float [B][H] (relu of lin_readout.0); score float [B][H]
+ * (before the normalisation).  Backward, byte offsets into the workspace: dh float [node_cap][hidden]
+ * (gradient of the layer output being processed; of the top layer after the Set2Set backward); dz, dout
+ * float [node_cap][hidden]; sv float [2][node_cap][nh] (sum of a * da | gradient of er); dx0 float
+ * [node_cap][64]; dgates float [T][K][B][4H] (pre-activation gate gradients); dy float [B][2][H]
+ * (lin_readout.0 | .2 output gradients).                                                              */
+typedef struct {
+  int64_t x0, z[8], h[8], att[8], qstar, hs, cs, gates, alpha, y1, score;
+  int64_t dh, dz, dout, sv, dx0, dgates, dy;
+} gccb_gat_stash_t;
+int gccb_gat_stash_layout(const gccb_gat_cfg_t* cfg, int32_t batch, int32_t node_cap,
+                          gccb_gat_stash_t* out /* host */);
+
 /* ---- contrastive head ------------------------------------------------------------------ */
 /* MemoryMoCo.forward logits (memory_moco.py:33-44): out[B][K+1] = [q.k | q.memory^T] / T */
 int gccb_moco_logits(const float* q, const float* k, const float* memory, int32_t B,

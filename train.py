@@ -73,7 +73,7 @@ def parse_option(argv=None):
     parser.add_argument("--graph-nodes", type=int, default=1000000)
     parser.add_argument("--graph-edges", type=int, default=20000000)
     # model definition
-    parser.add_argument("--model", type=str, default="gin", choices=["gin"])
+    parser.add_argument("--model", type=str, default="gin", choices=["gin", "gat"])
     parser.add_argument("--num-layer", type=int, default=5, help="gnn layers")
     parser.add_argument("--readout", type=str, default="avg", choices=["avg", "set2set"])
     parser.add_argument("--set2set-lstm-layer", type=int, default=3, help="lstm layers for s2s")
