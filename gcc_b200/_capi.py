@@ -113,6 +113,15 @@ _PROTOS = {
     "gccb_clip_adagrad_ema": (C.c_int, [p, p, p, p, C.c_int64, C.c_int64, p, C.c_float, C.c_float, C.c_float,
                                         C.c_float, C.c_float, p, p, p, C.c_int32, p]),
     "gccb_sum_ranks": (C.c_int, [p, C.c_int32, C.c_int64, C.c_int64, p, C.c_int64, p, p]),
+    "gccb_ft_head_workspace": (C.c_size_t, [C.c_int32, C.c_int32]),
+    "gccb_ft_head": (C.c_int, [p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, p, p, p, p, C.c_int64, C.c_int32,
+                               p, p, p, p, p, C.c_size_t, p]),
+    "gccb_clip_value_adam": (C.c_int, [p, p, p, p, C.c_int64, p, C.c_float, C.c_float, C.c_float, C.c_float,
+                                       C.c_float, p, C.c_int32, p]),
+    "gccb_clip_value_sgd": (C.c_int, [p, p, p, C.c_int64, p, C.c_float, C.c_float, C.c_float, p, C.c_int32, p]),
+    "gccb_clip_value_adagrad": (C.c_int, [p, p, p, C.c_int64, p, C.c_float, C.c_float, C.c_float, p, C.c_int32,
+                                          p]),
+    "gccb_gather_features": (C.c_int, [C.POINTER(GraphSet), p, C.POINTER(Batch), C.c_int32, p, C.c_int32, p, p]),
     "gccb_tc_gemm_bf16": (C.c_int, [p, p, C.c_int32, C.c_int32, C.c_int32, p, p, C.c_float, p, p, C.c_int32, p,
                                     C.c_int32, p, p]),
     "gccb_cast_bf16": (C.c_int, [p, C.c_int32, C.c_int32, C.c_int32, p, C.c_int32, C.c_int32, C.c_int32, p, p]),

@@ -143,6 +143,11 @@ __device__ __forceinline__ int warp_scan_incl(int v, int lane) {
   return v;
 }
 
+// a graph id of a gccb_graph_set_t taken from the caller: clamped, so that it never reads out of bounds
+__device__ __forceinline__ int64_t clamp_graph(int64_t id, int64_t n_graphs) {
+  return id < 0 ? 0 : (id >= n_graphs ? n_graphs - 1 : id);
+}
+
 // Block-wide exclusive scan of one int per thread (blockDim.x <= 1024, multiple of 32).
 // `scratch` must hold 33 ints of shared memory.  Returns exclusive prefix; *total = block sum.
 __device__ __forceinline__ int block_scan_excl(int v, int* scratch, int* total) {

@@ -12,10 +12,6 @@
 
 namespace gccb {
 
-__device__ __forceinline__ int64_t clamp_graph(int64_t id, int64_t n_graphs) {
-  return id < 0 ? 0 : (id >= n_graphs ? n_graphs - 1 : id);     // caller-supplied ids: never read out of bounds
-}
-
 // Pass 1: per-view exclusive scans of the picked graphs' sizes -> node_off / edge_off, counters (n, m, 0, 0) and
 // the capacity check (batch_offsets_kernel's contract: on overflow the view is published empty).
 // grid = 2 (views), block = 256.

@@ -18,16 +18,17 @@ gcc/datasets/data_util.py:35-113,227-236, train.py:516-545).
 The reference downloads its datasets; there is no network here, so `dataset` may also be an in-memory
 object -- (CSRGraph, labels) / (list[CSRGraph], labels) -- or a path.
 """
+import ctypes as C
 import os
 from collections import namedtuple
 
 import numpy as np
 import torch
 
-from .. import _lib
+from .. import _capi, _lib
 from . import synthetic
 from .data_util import BatchedSubgraphs
-from .graph_dataset import HOPCAP, BatchBuffers, DeviceGraph, LoadBalanceGraphDataset
+from .graph_dataset import HOPCAP, BatchBuffers, DeviceGraph, LoadBalanceGraphDataset, seed_first_union
 
 Data = namedtuple("Data", ["x", "edge_index", "y"])          # data_util.py:44
 
@@ -270,6 +271,7 @@ class NodeClassificationDatasetLabeled(_LabeledBase):
         self.num_classes = int(y.shape[1]) if y.ndim == 2 else int(self.labels.max()) + 1
         self.device = torch.device(device)
         _lib.require_device()
+        self.labels_dev = torch.from_numpy(self.labels).to(self.device)      # FinetuneEngine's label table
         # max_nodes_per_seed = rw_hops for every seed (:412): the degree formula capped at rw_hops
         self.graph = DeviceGraph(graph, rw_hops, restart_prob, int(seed), self.device, budget_exponent=1.0,
                                  budget_cap=rw_hops)
@@ -312,6 +314,17 @@ class NodeClassificationDatasetLabeled(_LabeledBase):
         buf.check_flags()
         return BatchedSubgraphs(buf, 0)
 
+    def device_batch(self, ids):
+        """_make_batch for the items `ids` (device int64 [b]) with no host sync: the same buffers, walks and
+        features.  A batch over its capacity is published empty with the buffers' flag raised; the caller reads
+        the flag."""
+        b = ids.numel()
+        buf = self._buffers(b)
+        first = self.next_sample
+        self.next_sample += b
+        LoadBalanceGraphDataset.sample_batch(self, first_sample=first, seeds=ids, buffers=buf)
+        return buf
+
     posenc = LoadBalanceGraphDataset.posenc
 
 
@@ -332,15 +345,22 @@ class GraphClassificationDatasetLabeled(_LabeledBase):
         self.length = self.total = len(graphs)
         assert len(self.labels) == self.length
         # the reference's self.dict (:355): every item is prepared once.  seed = argmax degree (:361, first
-        # maximum), moved to row 0
-        self.seeds = np.array([int(np.argmax(np.diff(g.indptr))) for g in graphs], dtype=np.int64)
-        self.items = [seed_first(g.indptr, g.indices, s)[:2] for g, s in zip(graphs, self.seeds)]
+        # maximum), moved to row 0; the relabelled items also form one union CSR (the gccb_graph_set_t layout)
+        self.seeds, self.items, indptr, indices, node_off, edge_off = seed_first_union(graphs)
         self.sizes = np.array([g.num_nodes for g in graphs], dtype=np.int64)
         self.nnz = np.array([len(g.indices) for g in graphs], dtype=np.int64)
         self.device = torch.device(device)
         _lib.require_device()
         self.batch_size = int(min(batch_size, self.length))
         self._bufs = {}
+        to = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a)).to(device=self.device, dtype=dt)
+        self.union_indptr, self.union_indices = to(indptr, torch.int64), to(indices, torch.int32)
+        self.node_off_host = node_off
+        self.union_node_off, self.union_edge_off = to(node_off, torch.int64), to(edge_off, torch.int64)
+        self.set_c = _capi.GraphSet(self.union_indptr.data_ptr(), self.union_indices.data_ptr(),
+                                    self.union_node_off.data_ptr(), self.union_edge_off.data_ptr(), self.length)
+        self.labels_dev = to(self.labels, torch.int64)                       # FinetuneEngine's label table
+        self._features = None
 
     @staticmethod
     def _load(dataset):
@@ -372,6 +392,43 @@ class GraphClassificationDatasetLabeled(_LabeledBase):
         _posenc(buf)
         buf.check_flags()
         return BatchedSubgraphs(buf, 0)
+
+    def feature_cache(self):
+        """Positional features of every vertex of the union, [total vertices][P], computed once on first use.  The
+        eigensolver is deterministic, so these are the rows _make_batch computes for a graph in any batch.  Built
+        from batches of consecutive ids, whose rows are the union's rows in order: one device copy per batch."""
+        if self._features is None:
+            P, B = self.positional_embedding_size, self.batch_size
+            no = self.node_off_host
+            cache = torch.empty(int(no[-1]), P, dtype=torch.float32, device=self.device)
+            full = self._buffers(B)
+            ids = torch.arange(self.length, dtype=torch.int64, device=self.device)
+            for a in range(0, self.length, B):
+                b = min(B, self.length - a)
+                buf = full.narrow(b)
+                _lib.check(_lib.get().gccb_gather_graphs(C.byref(self.set_c), _lib.dptr(ids[a:a + b]), C.byref(buf.c),
+                                                         _lib.stream_ptr()), "gccb_gather_graphs")
+                buf.node_off[1].zero_()                # view 1 absent for the eigensolver, as fill_whole_graphs
+                buf.edge_off[1].zero_()
+                buf.node_off[1, b] = -1
+                buf.counters[b:2 * b].zero_()
+                _posenc(buf)
+                cache[no[a]:no[a + b]].copy_(buf.pos[0, :no[a + b] - no[a]])
+            full.check_flags()
+            self._features = cache
+        return self._features
+
+    def device_batch(self, ids):
+        """_make_batch for the graphs `ids` (device int64 [b]) with no host sync: the union gather and the cached
+        features.  The buffers hold the b largest graphs, so a batch never overflows."""
+        buf = self._buffers(ids.numel())
+        lib, st = _lib.get(), _lib.stream_ptr()
+        _lib.check(lib.gccb_gather_graphs(C.byref(self.set_c), _lib.dptr(ids), C.byref(buf.c), st),
+                   "gccb_gather_graphs")
+        _lib.check(lib.gccb_gather_features(C.byref(self.set_c), _lib.dptr(ids), C.byref(buf.c), 0,
+                                            _lib.dptr(self.feature_cache()), buf.pos_dim, _lib.dptr(buf.pos), st),
+                   "gccb_gather_features")
+        return buf
 
 
 def labeled_batcher():

@@ -25,6 +25,91 @@ from .parallel import StepExchange, first_sample_id
 ADAGRAD_EPS = 1e-10                                    # torch.optim.Adagrad's default; train.py never sets it
 
 
+class FlatOptimizer:
+    """The state of one torch.optim.{Adam,SGD,Adagrad} over a flat fp32 buffer of n live entries, for the flat optimiser
+    kernels (csrc/optim.cu, csrc/finetune.cu): the moment / sum buffers, the step count t and the per-step `hyper`
+    scalars.  adam: betas, eps; sgd: momentum (dampening 0, no Nesterov); adagrad: lr_decay, eps 1e-10."""
+
+    def __init__(self, kind, n, device, lr, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-5, momentum=0.9,
+                 lr_decay=0.0):
+        if kind not in ("adam", "sgd", "adagrad"):
+            raise ValueError("optimizer must be adam, sgd or adagrad, not %r" % (kind,))
+        self.kind, self.lr0, self.betas, self.eps, self.wd = kind, lr, betas, eps, weight_decay
+        self.momentum, self.lr_decay = momentum, lr_decay
+        f32 = dict(dtype=torch.float32, device=device)
+        self.m = self.v = self.state = None
+        if kind == "adam":
+            self.m = torch.zeros(n, **f32)
+            self.v = torch.zeros(n, **f32)
+        elif kind == "adagrad" or momentum != 0:
+            # SGD's momentum_buffer or Adagrad's sum; zero is also torch's starting point (Adagrad's
+            # initial_accumulator_value 0; SGD's first-step copy, see csrc/optim_rules.cuh)
+            self.state = torch.zeros(n, **f32)
+        self.t = 0                                     # steps issued (skipped ones included)
+        self.hyper = torch.zeros(4, **f32)
+        # ring of pinned slots: the host enqueues several steps ahead of the device, and an async H2D copy
+        # reads its pinned source when it EXECUTES, so each step needs a slot of its own
+        self.hyper_host = torch.zeros(256, 4, dtype=torch.float32).pin_memory()
+
+    def next_step(self, lr):
+        """Count one more step and enqueue its scalars (LR at step t, bias corrections) into `hyper`, without a
+        host sync."""
+        self.t += 1
+        slot = self.hyper_host[self.t % self.hyper_host.shape[0]]
+        if self.kind == "adam":
+            b1, b2 = self.betas
+            slot[0] = lr
+            slot[1] = 1.0 - b1 ** self.t
+            slot[2] = math.sqrt(1.0 - b2 ** self.t)
+        elif self.kind == "sgd":
+            slot[0] = lr
+        else:                                          # torch.optim.Adagrad's clr, in double
+            slot[0] = lr / (1.0 + (self.t - 1) * self.lr_decay)
+        self.hyper.copy_(slot, non_blocking=True)
+
+    def state_dict(self, model):
+        """The flat buffers in the layout of torch.optim.{Adam,SGD,Adagrad}(model.parameters()).state_dict()
+        (train.py:659-678,752).  Adam: exp_avg / exp_avg_sq / step for the parameters that receive gradients (the
+        GIN path); the unused set2set / lin_readout tensors have no state, as in the reference where they never get
+        a gradient.  SGD: momentum_buffer for those parameters once a step has run, and no state without momentum.
+        Adagrad: state for every parameter, as torch creates it at construction -- the unused tensors keep step 0
+        and a zero sum."""
+        names = [n for n, _ in model.named_parameters()]
+        state = {}
+        for i, (n, prm) in enumerate(model.named_parameters()):
+            if n in model._slices:
+                o, shape = model._slices[n]
+                cnt = 1
+                for d_ in shape:
+                    cnt *= d_
+                if self.kind == "adam":
+                    state[i] = {"step": torch.tensor(float(self.t)),
+                                "exp_avg": self.m[o:o + cnt].view(shape).clone(),
+                                "exp_avg_sq": self.v[o:o + cnt].view(shape).clone()}
+                elif self.kind == "sgd":
+                    if self.state is not None and self.t > 0:
+                        state[i] = {"momentum_buffer": self.state[o:o + cnt].view(shape).clone()}
+                else:
+                    state[i] = {"step": torch.tensor(float(self.t)),
+                                "sum": self.state[o:o + cnt].view(shape).clone()}
+            elif self.kind == "adagrad":
+                state[i] = {"step": torch.tensor(0.0), "sum": torch.zeros_like(prm.detach())}
+        params = list(range(len(names)))
+        if self.kind == "adam":
+            group = {"lr": self.lr0, "betas": tuple(self.betas), "eps": self.eps, "weight_decay": self.wd,
+                     "amsgrad": False, "maximize": False, "foreach": None, "capturable": False,
+                     "differentiable": False, "fused": None, "params": params}
+        elif self.kind == "sgd":
+            group = {"lr": self.lr0, "momentum": self.momentum, "dampening": 0, "weight_decay": self.wd,
+                     "nesterov": False, "maximize": False, "foreach": None, "differentiable": False, "fused": None,
+                     "params": params}
+        else:
+            group = {"lr": self.lr0, "lr_decay": self.lr_decay, "eps": ADAGRAD_EPS, "weight_decay": self.wd,
+                     "initial_accumulator_value": 0, "foreach": None, "maximize": False, "differentiable": False,
+                     "fused": None, "params": params}
+        return {"state": state, "param_groups": [group]}
+
+
 class PretrainEngine:
     def __init__(self, dataset, model, model_ema, contrast, moco=True, learning_rate=0.005,
                  betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-5, clip_norm=1.0, alpha=0.999,
@@ -57,19 +142,7 @@ class PretrainEngine:
             self.xch = StepExchange(B, H, n_live, world_size, dev, process_group)
             self.payload = self.xch.payload
         self.grads = self.xch.grads_send if self.xch else torch.zeros(n_live, **f32)
-        self.adam_m = self.adam_v = self.opt_state = None
-        if optimizer == "adam":
-            self.adam_m = torch.zeros(n_live, **f32)
-            self.adam_v = torch.zeros(n_live, **f32)
-        elif optimizer == "adagrad" or momentum != 0:
-            # SGD's momentum_buffer or Adagrad's sum over the live parameters; zero is also torch's starting
-            # point (Adagrad's initial_accumulator_value 0; SGD's first-step copy, see csrc/optim.cu)
-            self.opt_state = torch.zeros(n_live, **f32)
-        self.adam_t = 0                                # steps issued (skipped ones included), every optimiser
-        self.hyper = torch.zeros(4, **f32)
-        # ring of pinned slots: the host enqueues several steps ahead of the device, and an async H2D copy
-        # reads its pinned source when it EXECUTES, so each step needs a slot of its own
-        self.hyper_host = torch.zeros(256, 4, dtype=torch.float32).pin_memory()
+        self.opt = FlatOptimizer(optimizer, n_live, dev, learning_rate, betas, eps, weight_decay, momentum, lr_decay)
         # loss, prob, grad_norm(pre-clip), overflow marker of this rank's batch (multi-GPU skip protocol)
         self.stats = self.xch.stats_send if self.xch else torch.zeros(4, **f32)
         self.stats_acc = torch.zeros(4, dtype=torch.float64, device=dev)   # per-step sums since the last read_stats()
@@ -128,19 +201,12 @@ class PretrainEngine:
     def _new_stream(self, group, priority):
         return torch.cuda.Stream(device=self.dev, priority=priority)
 
-    def _hyper(self, lr):
-        self.adam_t += 1
-        slot = self.hyper_host[self.adam_t % self.hyper_host.shape[0]]
-        if self.optimizer == "adam":
-            b1, b2 = self.betas
-            slot[0] = lr
-            slot[1] = 1.0 - b1 ** self.adam_t
-            slot[2] = math.sqrt(1.0 - b2 ** self.adam_t)
-        elif self.optimizer == "sgd":
-            slot[0] = lr
-        else:                                          # torch.optim.Adagrad's clr, in double
-            slot[0] = lr / (1.0 + (self.adam_t - 1) * self.lr_decay)
-        self.hyper.copy_(slot, non_blocking=True)
+    # the optimiser state under its historical names (tests and tools read them)
+    adam_m = property(lambda self: self.opt.m)
+    adam_v = property(lambda self: self.opt.v)
+    opt_state = property(lambda self: self.opt.state)
+    adam_t = property(lambda self: self.opt.t)
+    hyper = property(lambda self: self.opt.hyper)
 
     def _prepare(self, seeds):
         """Issue sampler + eigensolver of batch number `self.prepared` on the data stream."""
@@ -273,7 +339,7 @@ class PretrainEngine:
                                           n_live + 3, _lib.dptr(self.any_skip), st), "gccb_sum_ranks")
             scale = 1.0 / self.world
             skip_word, skip_mask = _lib.dptr(self.any_skip), -1     # every replica skips the same steps
-        self._hyper(lr)
+        self.opt.next_step(lr)
         p_ema, alpha = (_lib.dptr(ema.flat_params), self.alpha) if self.moco else (None, -1.0)
         tail = (p_ema, model.n_live, model._n_all, _lib.dptr(self.hyper))
         common = (self.wd, self.clip, alpha, scale, C.c_void_p(self.stats.data_ptr() + 8), _lib.dptr(self.norm_ws),
@@ -338,43 +404,5 @@ class PretrainEngine:
                     window_grad_norm=acc[2] / w)
 
     def optimizer_state_dict(self):
-        """The flat optimiser buffers in the layout of torch.optim.{Adam,SGD,Adagrad}(model.parameters())
-        .state_dict() (train.py:659-678,752).  Adam: exp_avg / exp_avg_sq / step for the parameters that receive
-        gradients (the GIN path); the unused set2set / lin_readout tensors have no state, as in the reference
-        where they never get a gradient.  SGD: momentum_buffer for those parameters once a step has run, and
-        no state without momentum.  Adagrad: state for every parameter, as torch creates it at construction --
-        the unused tensors keep step 0 and a zero sum."""
-        names = [n for n, _ in self.model.named_parameters()]
-        state = {}
-        for i, (n, prm) in enumerate(self.model.named_parameters()):
-            if n in self.model._slices:
-                o, shape = self.model._slices[n]
-                cnt = 1
-                for d_ in shape:
-                    cnt *= d_
-                if self.optimizer == "adam":
-                    state[i] = {"step": torch.tensor(float(self.adam_t)),
-                                "exp_avg": self.adam_m[o:o + cnt].view(shape).clone(),
-                                "exp_avg_sq": self.adam_v[o:o + cnt].view(shape).clone()}
-                elif self.optimizer == "sgd":
-                    if self.opt_state is not None and self.adam_t > 0:
-                        state[i] = {"momentum_buffer": self.opt_state[o:o + cnt].view(shape).clone()}
-                else:
-                    state[i] = {"step": torch.tensor(float(self.adam_t)),
-                                "sum": self.opt_state[o:o + cnt].view(shape).clone()}
-            elif self.optimizer == "adagrad":
-                state[i] = {"step": torch.tensor(0.0), "sum": torch.zeros_like(prm.detach())}
-        params = list(range(len(names)))
-        if self.optimizer == "adam":
-            group = {"lr": self.lr0, "betas": tuple(self.betas), "eps": self.eps, "weight_decay": self.wd,
-                     "amsgrad": False, "maximize": False, "foreach": None, "capturable": False,
-                     "differentiable": False, "fused": None, "params": params}
-        elif self.optimizer == "sgd":
-            group = {"lr": self.lr0, "momentum": self.momentum, "dampening": 0, "weight_decay": self.wd,
-                     "nesterov": False, "maximize": False, "foreach": None, "differentiable": False, "fused": None,
-                     "params": params}
-        else:
-            group = {"lr": self.lr0, "lr_decay": self.lr_decay, "eps": ADAGRAD_EPS, "weight_decay": self.wd,
-                     "initial_accumulator_value": 0, "foreach": None, "maximize": False, "differentiable": False,
-                     "fused": None, "params": params}
-        return {"state": state, "param_groups": [group]}
+        """FlatOptimizer.state_dict of the encoder's optimiser."""
+        return self.opt.state_dict(self.model)

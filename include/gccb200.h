@@ -358,6 +358,38 @@ int gccb_clip_adagrad_ema(float* p, float* g, float* sum, float* p_ema, int64_t 
 int gccb_sum_ranks(const float* gathered, int32_t world, int64_t stride, int64_t n, float* out,
                    int64_t flag_index, int32_t* any_flag_out, gccb_stream_t stream);
 
+/* ---- supervised finetuning (csrc/finetune.cu) ------------------------------------------------------
+ * Classification head (train.py:219-241): logits = feat W^T + bias over the first b rows of feat [B][H],
+ * W [C][H], bias [C]; row i's label is labels[item_ids[i]] (device int64 tables, ids clamped to n_items).
+ * stats (device, 3 floats): mean cross-entropy (max-subtracted log-sum-exp), the count of rows whose FIRST
+ * maximum logit is the label (torch.argmax's tie rule; correct / b is the micro-F1), b.  Unless eval != 0 also
+ * dlogits = (softmax - onehot(y)) / b, dfeat [b][H] = dlogits W, dW [C][H] = dlogits^T feat, db [C] = column sums
+ * of dlogits.  H in {32, 64, 128, 256}, 2 <= C <= 128, 0 < b <= B <= 4096, else GCCB_ERR_BADARG.  No float
+ * atomics: every sum over rows runs in a fixed order, so the call is bit-identical from run to run.          */
+size_t gccb_ft_head_workspace(int32_t B, int32_t C);
+int gccb_ft_head(const float* feat, int32_t B, int32_t b, int32_t H, int32_t C, const float* W, const float* bias,
+                 const int64_t* item_ids, const int64_t* labels, int64_t n_items, int32_t eval, float* dfeat,
+                 float* dW, float* db, float* stats, void* workspace, size_t workspace_bytes, gccb_stream_t stream);
+/* clip_grad_value_(params, clip_value) (train.py:227-228) then the optimiser step over n floats: g is clamped to
+ * [-clip_value, clip_value] (g itself is not written), then the update of gccb_clip_{adam,sgd,adagrad}_ema after
+ * its norm clip -- the same weight decay, state buffers and `hyper` layout.  No EMA, no norm.  skip_word /
+ * skip_mask: as for gccb_moco_enqueue, the call is a no-op for a batch published empty.                      */
+int gccb_clip_value_adam(float* p, const float* g, float* m, float* v, int64_t n, const float* hyper, float beta1,
+                         float beta2, float eps, float weight_decay, float clip_value, const int32_t* skip_word,
+                         int32_t skip_mask, gccb_stream_t stream);
+int gccb_clip_value_sgd(float* p, const float* g, float* buf, int64_t n, const float* hyper, float momentum,
+                        float weight_decay, float clip_value, const int32_t* skip_word, int32_t skip_mask,
+                        gccb_stream_t stream);
+int gccb_clip_value_adagrad(float* p, const float* g, float* sum, int64_t n, const float* hyper, float eps,
+                            float weight_decay, float clip_value, const int32_t* skip_word, int32_t skip_mask,
+                            gccb_stream_t stream);
+/* Positional features of a whole-graph batch built by gccb_gather_graphs from `set`, copied from a per-vertex
+ * cache [total vertices of set][pos_dim]: row r of batch graph g in view `view` gets cache row
+ * set->node_off[graph_ids[g]] + (r - batch->node_off[view][g]).  pos is [2][node_cap][pos_dim].  A view published
+ * empty is left alone.  No workspace, no host sync.                                                          */
+int gccb_gather_features(const gccb_graph_set_t* set, const int64_t* graph_ids, const gccb_batch_t* batch,
+                         int32_t view, const float* cache, int32_t pos_dim, float* pos, gccb_stream_t stream);
+
 /* ---- tensor-core contraction (wgmma + TMA; csrc/tc_gemm.cu) ---------------------------------------
  * The dense products of the path at hidden >= 128 (BASELINE config 4): the GIN MLP's Linear layers
  * (gcc/models/gin.py:107-116) with the BatchNorm column statistics of :115 fused into the epilogue,

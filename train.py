@@ -18,11 +18,14 @@ step run on the GPU through gcc_b200.engine.PretrainEngine (no DataLoader worker
 loss / prob / grad-norm are accumulated on the device EVERY step and read every --print-freq steps, so
 the meters average over all steps like the reference's).
 
-Fine-tuning (--finetune, train.py:175-337,516-545,631-660,788-792 of the reference): train_finetune /
-test_finetune keep the reference's signatures and arithmetic -- GraphEncoder forward/backward through the
-same device kernels (autograd Function), torch's Linear head, CrossEntropyLoss, clip_grad_value_(1), the
---optimizer for the encoder and Adam for the output layer, micro-F1 per batch -- over the labeled datasets of gcc_b200/datasets/labeled.py,
-split by the reference's StratifiedKFold(10, shuffle, seed)[fold_idx].
+Fine-tuning (--finetune, train.py:175-337,516-545,631-660,788-792 of the reference): main_finetune drives
+gcc_b200.finetune.FinetuneEngine -- every step on the device with no host sync: the batch, the encoder, the head's
+cross-entropy and micro-F1, clip_grad_value_(1), the --optimizer for the encoder and Adam for the output layer --
+over the labeled datasets of gcc_b200/datasets/labeled.py, split by the reference's StratifiedKFold(10, shuffle,
+seed)[fold_idx].  train_finetune / test_finetune keep the reference's signatures and torch-ops arithmetic
+(GraphEncoder forward/backward through the same device kernels as an autograd Function, torch's Linear head,
+CrossEntropyLoss, torch.optim): they compute the same steps on the same batches and are what the engine is tested
+against.
 
     python train.py --finetune --dataset usa_airport --resume saved/.../current.pth --epochs 30 --fold-idx 0
 """
@@ -38,6 +41,7 @@ from gcc_b200.datasets import downstream, synthetic
 from gcc_b200.datasets.graph_dataset import (GraphClassificationDataset, LoadBalanceGraphDataset,
                                              NodeClassificationDataset)
 from gcc_b200.engine import PretrainEngine
+from gcc_b200.finetune import FinetuneEngine
 from gcc_b200.models import GraphEncoder
 from gcc_b200.utils.misc import AverageMeter, warmup_linear
 
@@ -365,23 +369,23 @@ def main_finetune(args, dataset=None):
     idx_list = list(skf.split(np.zeros(len(labels)), labels))
     assert 0 <= args.fold_idx < 10, "fold_idx must be from 0 to 9."
     train_idx, test_idx = idx_list[args.fold_idx]
-    train_loader = LabeledLoader(dataset, train_idx, args.batch_size, shuffle=True, seed=args.seed)
-    valid_loader = LabeledLoader(dataset, test_idx, args.batch_size, shuffle=False)
     model = _make_encoder(args)
     if checkpoint is not None:
         model.load_state_dict(checkpoint["model"])
     model = model.to(dev)
-    criterion = torch.nn.CrossEntropyLoss()
     output_layer = torch.nn.Linear(in_features=args.hidden_size, out_features=dataset.num_classes).to(dev)
-    output_layer_optimizer = torch.optim.Adam(output_layer.parameters(), lr=args.learning_rate,
-                                              betas=(args.beta1, args.beta2), weight_decay=args.weight_decay)
 
     def clear_bn(m):                                       # train.py:648-653
         if m.__class__.__name__.find("BatchNorm") != -1:
             m.reset_running_stats()
 
     model.apply(clear_bn)
-    optimizer = make_optimizer(args, model.parameters())
+    # the --optimizer for the encoder, Adam for the output layer, both after clip_grad_value_(1), every step on the
+    # device (gcc_b200/finetune.py); train_finetune / test_finetune are the same steps with torch ops
+    engine = FinetuneEngine(dataset, model, output_layer, optimizer=args.optimizer, lr=args.learning_rate,
+                            betas=(args.beta1, args.beta2), weight_decay=args.weight_decay, momentum=args.momentum,
+                            lr_decay=args.lr_decay_rate, batch_size=args.batch_size)
+    rng = np.random.RandomState(args.seed)                 # LabeledLoader's shuffle: one permutation per epoch
     sw = None
     try:
         from torch.utils.tensorboard import SummaryWriter
@@ -391,14 +395,15 @@ def main_finetune(args, dataset=None):
     epoch = 0
     for epoch in range(1, args.epochs + 1):
         t0 = time.time()
-        loss, _ = train_finetune(epoch, train_loader, model, output_layer, criterion, optimizer,
-                                 output_layer_optimizer, sw, args)
+        loss, _ = engine.train_epoch(epoch, rng.permutation(np.asarray(train_idx, dtype=np.int64)), args.epochs,
+                                     sw=sw, print_freq=args.print_freq, tb_freq=args.tb_freq)
         print("epoch {}, loss {:.4f}, total time {:.2f}".format(epoch, loss, time.time() - t0))
-        state = {"opt": args, "model": model.state_dict(), "optimizer": optimizer.state_dict(), "epoch": epoch}
+        state = {"opt": args, "model": model.state_dict(), "optimizer": engine.optimizer_state_dict(),
+                 "epoch": epoch}
         torch.save(state, os.path.join(args.model_folder, "current.pth"))
         if epoch % args.save_freq == 0:
             torch.save(state, os.path.join(args.model_folder, "ckpt_epoch_{epoch}.pth".format(epoch=epoch)))
-    _, valid_f1 = test_finetune(epoch, valid_loader, model, output_layer, criterion, sw, args)
+    _, valid_f1 = engine.evaluate(epoch, test_idx, sw)
     return valid_f1
 
 
