@@ -78,6 +78,12 @@ _PROTOS = {
     "gccb_draw_seeds": (C.c_int, [p, C.c_int64, C.c_uint64, C.c_int64, C.c_int32, p, p, p]),
     "gccb_sample_batch_workspace": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32]),
     "gccb_sample_batch": (C.c_int, [C.POINTER(Graph), p, p, C.POINTER(Batch), p, C.c_size_t, p]),
+    "gccb_pair_seeds": (C.c_int, [C.POINTER(Graph), p, C.c_int32, p, p, C.c_int32, p, p]),
+    "gccb_sample_batch_pairs": (C.c_int, [C.POINTER(Graph), p, p, p, C.POINTER(Batch), p, C.c_size_t, p]),
+    "gccb_ns_ego_cap": (C.c_int32, [C.c_int32]),
+    "gccb_ns_batch_workspace": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32]),
+    "gccb_ns_batch": (C.c_int, [C.POINTER(Graph), p, p, p, C.c_int32, C.c_int32, C.POINTER(Batch), p, C.c_size_t,
+                                p]),
     "gccb_gather_graphs": (C.c_int, [C.POINTER(GraphSet), p, C.POINTER(Batch), p]),
     "gccb_posenc_workspace": (C.c_size_t, [C.c_int32, C.c_int32]),
     "gccb_posenc": (C.c_int, [C.POINTER(Batch), C.c_int32, C.c_int32, p, p, p, C.c_size_t, p]),

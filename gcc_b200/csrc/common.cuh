@@ -79,6 +79,9 @@ inline void ensure_dyn_smem(K kern, size_t bytes) {
 #define GCCB_TAG_SEED 1u
 #define GCCB_TAG_DROPOUT 2u
 #define GCCB_TAG_PRONE 3u
+#define GCCB_TAG_STEP 4u       // step_dist draw of the key view (hop 0)
+#define GCCB_TAG_KHOP 5u       // hops of the key seed's plain walk (hop = 1, 2)
+#define GCCB_TAG_NS 6u         // neighbour sampling (aug="ns"): high byte of the hop in the tag's high byte
 
 // device status flag bits (gccb200.h: GCCB_FLAG_*)
 namespace gccb {

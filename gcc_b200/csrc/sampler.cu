@@ -96,36 +96,149 @@ __device__ __forceinline__ int adj_count(const int32_t* __restrict__ indices, in
 #endif
 #define GCCB_HIT_STAGE 128     // hits of one row parked in shared memory before their pool slot is known
 
-// Pass 1: walk + sort/unique + induced-degree count.  grid = 2B, block = GCCB_ST.
-// dyn smem: keys[P] ints, P = pow2 >= max_budget + HOPCAP.
-__global__ void __launch_bounds__(GCCB_ST)
-rwr_walk_unique_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices, int64_t n_nodes,
-                       const int32_t* __restrict__ budget_table, int budget_table_len,
-                       uint32_t restart_thresh, uint64_t key, const int64_t* __restrict__ seeds,
-                       const int64_t* __restrict__ sample_ids, int B, int cap_n,
-                       int32_t* __restrict__ subv_scratch, int32_t* __restrict__ subdeg_scratch,
-                       int32_t* __restrict__ rowstart_scratch, int32_t* __restrict__ pool, int pool_cap,
-                       unsigned long long* __restrict__ pool_counter,
-                       int64_t* __restrict__ counters, int32_t* __restrict__ flags) {
-  GCCB_DYN_SMEM(int, keys);
-  __shared__ int scan_scratch[33];
-  __shared__ int stage[GCCB_SW][GCCB_HIT_STAGE];      // per-warp parking of one row's hits
-  __shared__ int s_tstar, s_m;
-  __shared__ unsigned long long s_sumdeg;
-  __shared__ int s_nhub, s_pos;
-  __shared__ unsigned bloom[GCCB_BLOOM_WORDS];        // one-hash membership filter of the frontier (8 KB)
-  __shared__ int hub_rows[GCCB_HUB_LIST];             // hub rows of this ego-net: probed by the whole CTA
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int slot = blockIdx.x;            // view-major: slot = view * B + g
-  const int view = slot / B, g = slot - view * B;
-  int64_t seed64 = seeds[g];
-  seed64 = seed64 < 0 ? 0 : (seed64 >= n_nodes ? n_nodes - 1 : seed64);   // caller-supplied seeds: never read out of bounds
-  const int seed = (int)seed64;
-  const uint64_t sample = (uint64_t)sample_ids[g];
-  int64_t sdeg = indptr[seed64 + 1] - indptr[seed64];
-  const int budget = budget_table[sdeg < budget_table_len ? (int)sdeg : budget_table_len - 1];
+// Block-wide ascending bitonic sort of a[0..cnt), padded with INT_MAX to a power of two (the buffer must hold it).
+__device__ void block_sort_pad(int* a, int cnt) {
+  const int tid = threadIdx.x;
+  int P = 1;
+  while (P < cnt) P <<= 1;
+  for (int i = cnt + tid; i < P; i += GCCB_ST) a[i] = 0x7fffffff;
+  __syncthreads();
+  for (int k = 2; k <= P; k <<= 1) {
+    for (int j = k >> 1; j > 0; j >>= 1) {
+      for (int i = tid; i < P; i += GCCB_ST) {
+        const int ixj = i ^ j;
+        if (ixj > i) {
+          const int x = a[i], y = a[ixj];
+          if ((x > y) == ((i & k) == 0)) { a[i] = y; a[ixj] = x; }
+        }
+      }
+      __syncthreads();
+    }
+  }
+}
 
-  if (tid == 0) { s_tstar = 0x7fffffff; s_m = 0; s_sumdeg = 0ull; }
+__device__ __forceinline__ bool in_sorted(const int* a, int n, int u) {
+  int lo = 0, hi = n;
+  while (lo < hi) { const int mid = (lo + hi) >> 1; if (a[mid] < u) lo = mid + 1; else hi = mid; }
+  return lo < n && a[lo] == u;
+}
+
+// Neighbour-sampled ego-net of `seed` (aug="ns", reference graph_dataset.py:131-162), built in shared memory:
+//   V[cap]  the union of all layers so far, ascending (the seed included);
+//   F[cap]  the current layer, ascending (a vertex's position in it keys its draws);
+//   S[Ps]   candidates of the next layer, then the merge buffer (Ps = pow2 >= max(k, 2) * cap >= k |F|, 2 cap).
+// Layer h = the de-duplicated union over u of layer h-1 of all neighbour entries of u if deg(u) <= k, else k distinct
+// entries drawn without replacement (Floyd's algorithm: draw t of u uses Philox (sample, position of u | t << 16,
+// hop, view, GCCB_TAG_NS)).  A layer is not reduced by the earlier ones: only the final union is.  The loop stops
+// early when a layer is empty or when V is closed under neighbourhood (every later layer then lies inside V); a
+// layer that merely adds nothing new does not stop it, because the next one draws afresh.
+// Writes subv = [seed, V \ {seed} ascending] and returns |V|, or -1 when |V| would exceed cap.  *layers = layers
+// expanded.  Every return value is uniform over the block.
+__device__ int ns_expand(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices, uint64_t key,
+                         uint64_t sample, uint32_t view, int seed, int hops, int k, int cap, int* V, int* F, int* S,
+                         int* scan_scratch, int32_t* __restrict__ subv, int* layers) {
+  __shared__ int s_miss;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  int nV = 1, nF = 1, checked = 0, hop = 1;
+  if (tid == 0) { V[0] = seed; F[0] = seed; }
+  __syncthreads();
+  for (; hop <= hops; ++hop) {
+    const uint32_t c3hop = (uint32_t)hop & 0xffu, c3tag = GCCB_TAG_NS | (((uint32_t)hop >> 8) << 8);
+    // candidates: min(deg, k) entries per vertex of the layer, at the vertex's offset in S
+    int nc = 0;
+    for (int b0 = 0; b0 < nF; b0 += GCCB_ST) {
+      const int i = b0 + tid;
+      int64_t beg = 0, d = 0;
+      if (i < nF) { beg = indptr[F[i]]; d = indptr[F[i] + 1] - beg; }
+      int tot;
+      const int ex = block_scan_excl(d <= k ? (int)d : k, scan_scratch, &tot);
+      if (i < nF) {
+        int* out = S + nc + ex;
+        if (d <= k) {
+          for (int e = 0; e < (int)d; ++e) out[e] = indices[beg + e];
+        } else {
+          for (int t = 0; t < k; ++t) {                   // entry positions: k distinct of [0, d)
+            const uint32_t j = (uint32_t)(d - k + t);
+            const u32x4 w = philox_at(key, sample, (uint32_t)i | ((uint32_t)t << 16), c3hop, view, c3tag);
+            const int r = (int)__umulhi(w.x, j + 1u);
+            bool dup = false;
+            for (int q = 0; q < t; ++q) dup |= out[q] == r;
+            out[t] = dup ? (int)j : r;
+          }
+          for (int t = 0; t < k; ++t) out[t] = indices[beg + out[t]];
+        }
+      }
+      nc += tot;
+    }
+    __syncthreads();
+    block_sort_pad(S, nc);
+    // the layer: unique candidates
+    int nF2 = 0;
+    for (int b0 = 0; b0 < nc; b0 += GCCB_ST) {
+      const int i = b0 + tid;
+      const int head = i < nc && (i == 0 || S[i - 1] != S[i]);
+      int tot;
+      const int ex = block_scan_excl(head, scan_scratch, &tot);
+      if (head && nF2 + ex < cap) F[nF2 + ex] = S[i];
+      nF2 += tot;
+    }
+    if (nF2 > cap) return -1;                             // the layer alone: so would be the union
+    nF = nF2;
+    __syncthreads();
+    if (nF == 0) break;
+    // new vertices of the union, appended to a copy of V and merged by a sort
+    int nNew = 0;
+    for (int b0 = 0; b0 < nF; b0 += GCCB_ST) {
+      const int i = b0 + tid;
+      const int fresh = i < nF && !in_sorted(V, nV, F[i]);
+      int tot;
+      const int ex = block_scan_excl(fresh, scan_scratch, &tot);
+      if (fresh) S[nV + nNew + ex] = F[i];
+      nNew += tot;
+    }
+    if (nV + nNew > cap) return -1;
+    if (nNew > 0) {
+      for (int i = tid; i < nV; i += GCCB_ST) S[i] = V[i];
+      block_sort_pad(S, nV + nNew);                       // (syncs before it reads)
+      nV += nNew;
+      for (int i = tid; i < nV; i += GCCB_ST) V[i] = S[i];
+      __syncthreads();
+    } else if (nV != checked) {
+      // nothing new: stop if no neighbour entry of V lies outside V (one look per size of V)
+      if (tid == 0) s_miss = 0;
+      __syncthreads();
+      int miss = 0;
+      for (int i = warp; i < nV; i += GCCB_SW) {
+        const int64_t end = indptr[V[i] + 1];
+        for (int64_t e = indptr[V[i]] + lane; e < end && !miss; e += 32) miss = !in_sorted(V, nV, indices[e]);
+      }
+      if (miss) s_miss = 1;
+      __syncthreads();
+      const bool closed = s_miss == 0;
+      __syncthreads();
+      if (closed) break;
+      checked = nV;
+    }
+  }
+  *layers = hop > hops ? hops : hop;
+  for (int i = tid; i < nV; i += GCCB_ST) {
+    const int v = V[i];
+    subv[v < seed ? i + 1 : (v == seed ? 0 : i)] = v;
+  }
+  return nV;
+}
+
+// RWR node set of one (sample, view) (reference graph_dataset.py:113-130, data_util.py:221-226): the traces from
+// seed64 until `budget` vertices are recorded, sorted and uniqued in keys[]; writes subv[1..n) = the visited vertices
+// but the seed, ascending, and returns n (the caller writes subv[0] = seed).  *steps = recorded vertices.  s_tstar
+// and s_m are the kernel's shared words (s_m is left 0).
+__device__ __forceinline__ int rwr_node_set(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices,
+                                            int budget, uint32_t restart_thresh, uint64_t key, uint64_t sample,
+                                            int view, int64_t seed64, int seed, int* keys, int* scan_scratch,
+                                            int* s_tstar, int* s_m, int32_t* __restrict__ flags,
+                                            int32_t* __restrict__ subv, int* steps) {
+  const int tid = threadIdx.x;
+  if (tid == 0) *s_tstar = 0x7fffffff;
   __syncthreads();
 
   // ---- phase A+B: trace lengths (RNG only), stopping trace, parallel walk ------------
@@ -142,9 +255,9 @@ rwr_walk_unique_kernel(const int64_t* __restrict__ indptr, const int32_t* __rest
     int chunk_total;
     int excl = block_scan_excl(len, scan_scratch, &chunk_total);
     int cum = base + excl + len;           // inclusive cumulative count after trace t
-    if (cum >= budget && cum - len < budget) s_tstar = (int)t;   // exactly one thread
+    if (cum >= budget && cum - len < budget) *s_tstar = (int)t;   // exactly one thread
     __syncthreads();
-    const int tstar = s_tstar;
+    const int tstar = *s_tstar;
     if ((int)t <= tstar) {
       // walk this trace; its nodes land at keys[base+excl .. +len)
       int64_t cur = seed64;
@@ -160,16 +273,16 @@ rwr_walk_unique_kernel(const int64_t* __restrict__ indptr, const int32_t* __rest
     }
     if (tstar != 0x7fffffff) {
       // total = cumulative count after trace tstar (held by the thread that owns it)
-      if ((int)t == tstar) s_m = cum;
+      if ((int)t == tstar) *s_m = cum;
       __syncthreads();
-      total = s_m;
+      total = *s_m;
       break;
     }
     base += chunk_total;
     __syncthreads();
   }
   __syncthreads();
-  if (tid == 0) s_m = 0;
+  if (tid == 0) *s_m = 0;
 
   // ---- phase C: bitonic sort of keys[0..total), padded to a power of two --------------
   int P = 1;
@@ -190,7 +303,6 @@ rwr_walk_unique_kernel(const int64_t* __restrict__ indptr, const int32_t* __rest
     }
   }
   // ---- unique, drop the seed; subv = [seed] + sorted rest (data_util.py:221-226) -------
-  int32_t* subv = subv_scratch + (size_t)slot * cap_n;
   int n_rest = 0;
   for (int b0 = 0; b0 < total; b0 += GCCB_ST) {
     int i = b0 + tid;
@@ -204,7 +316,74 @@ rwr_walk_unique_kernel(const int64_t* __restrict__ indptr, const int32_t* __rest
     if (head) subv[1 + n_rest + ex] = v;
     n_rest += cnt;
   }
-  const int n = n_rest + 1;
+  *steps = total;
+  return n_rest + 1;
+}
+
+enum { kModeRwr = 0, kModePairs = 1, kModeNs = 2 };
+
+// Pass 1: walk + sort/unique + induced-degree count.  grid = 2B, block = GCCB_ST.
+// dyn smem: keys[P] ints, P = pow2 >= max_budget + HOPCAP.
+// kMode = kModeRwr: both views walk from seeds[g] (gccb_sample_batch).  kModePairs: view 1 walks from and induces
+// around seeds_k[g]; both budgets come from seeds[g]'s degree.  kModeNs: the node set is ns_expand's from seeds[g] /
+// seeds_k[g] (dyn smem: its V, F and S, ns_cap = cap_n); a view over cap_n vertices is counted node_cap + 1 vertices,
+// no edges, so that batch_offsets_kernel publishes the view empty.  The arguments after `flags` are unused by kModeRwr.
+template <int kMode>
+__global__ void __launch_bounds__(GCCB_ST)
+rwr_walk_unique_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices, int64_t n_nodes,
+                       const int32_t* __restrict__ budget_table, int budget_table_len,
+                       uint32_t restart_thresh, uint64_t key, const int64_t* __restrict__ seeds,
+                       const int64_t* __restrict__ sample_ids, int B, int cap_n,
+                       int32_t* __restrict__ subv_scratch, int32_t* __restrict__ subdeg_scratch,
+                       int32_t* __restrict__ rowstart_scratch, int32_t* __restrict__ pool, int pool_cap,
+                       unsigned long long* __restrict__ pool_counter,
+                       int64_t* __restrict__ counters, int32_t* __restrict__ flags,
+                       const int64_t* __restrict__ seeds_k, int ns_hops, int ns_k, int node_cap) {
+  GCCB_DYN_SMEM(int, keys);
+  __shared__ int scan_scratch[33];
+  __shared__ int stage[GCCB_SW][GCCB_HIT_STAGE];      // per-warp parking of one row's hits
+  __shared__ int s_tstar, s_m;
+  __shared__ unsigned long long s_sumdeg;
+  __shared__ int s_nhub, s_pos;
+  __shared__ unsigned bloom[GCCB_BLOOM_WORDS];        // one-hash membership filter of the frontier (8 KB)
+  __shared__ int hub_rows[GCCB_HUB_LIST];             // hub rows of this ego-net: probed by the whole CTA
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int slot = blockIdx.x;            // view-major: slot = view * B + g
+  const int view = slot / B, g = slot - view * B;
+  int64_t seed64 = seeds[g];
+  seed64 = seed64 < 0 ? 0 : (seed64 >= n_nodes ? n_nodes - 1 : seed64);   // caller-supplied seeds: never read out of bounds
+  const int64_t q64 = seed64;
+  if constexpr (kMode != kModeRwr) {
+    if (view == 1) {
+      seed64 = seeds_k[g];
+      seed64 = seed64 < 0 ? 0 : (seed64 >= n_nodes ? n_nodes - 1 : seed64);
+    }
+  }
+  const int seed = (int)seed64;
+  const uint64_t sample = (uint64_t)sample_ids[g];
+  int32_t* subv = subv_scratch + (size_t)slot * cap_n;
+  if (tid == 0) { s_m = 0; s_sumdeg = 0ull; }
+  int n, total = 0;                                       // total: counters[2] (walk steps / ns layers expanded)
+  if constexpr (kMode == kModeNs) {
+    n = ns_expand(indptr, indices, key, sample, (uint32_t)view, seed, ns_hops, ns_k, cap_n, keys, keys + cap_n,
+                  keys + 2 * cap_n, scan_scratch, subv, &total);
+    if (n < 0) {                                          // too large: the whole view is published empty
+      if (tid == 0) {
+        counters[(size_t)slot * 4 + 0] = (int64_t)node_cap + 1;
+        counters[(size_t)slot * 4 + 1] = 0;
+        counters[(size_t)slot * 4 + 2] = total;
+        counters[(size_t)slot * 4 + 3] = 0;
+        atomicOr(flags, (int)GCCB_FLAG_NODE_OVERFLOW);
+      }
+      return;
+    }
+    __syncthreads();                                      // subv complete before it is copied to keys
+  } else {
+    const int64_t sdeg = indptr[q64 + 1] - indptr[q64];   // the budget's seed: the q view's
+    const int budget = budget_table[sdeg < budget_table_len ? (int)sdeg : budget_table_len - 1];
+    n = rwr_node_set(indptr, indices, budget, restart_thresh, key, sample, view, seed64, seed, keys, scan_scratch,
+                     &s_tstar, &s_m, flags, subv, &total);
+  }
   if (tid == 0) subv[0] = seed;
   __syncthreads();                       // global writes of this block visible to the block
   for (int i = tid; i < n; i += GCCB_ST) keys[i] = subv[i];
@@ -526,6 +705,33 @@ induce_fill_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict
   }
 }
 
+// One thread per sample: step ~ step_dist (first index with cdf > u, 53 Philox bits, GCCB_TAG_STEP), then `step`
+// uniform hops of a plain walk from seeds_q[i] (hop h: GCCB_TAG_KHOP, hop field h).  A vertex without neighbours ends
+// the walk where it is.
+__global__ void pair_seeds_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices,
+                                  int64_t n_nodes, uint64_t key, double cdf0, double cdf1, int n_steps,
+                                  const int64_t* __restrict__ seeds_q, const int64_t* __restrict__ sample_ids,
+                                  int count, int64_t* __restrict__ seeds_k) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= count) return;
+  const uint64_t sample = (uint64_t)sample_ids[i];
+  const u32x4 w = philox_at(key, sample, 0, 0, 0, GCCB_TAG_STEP);
+  const double u = (double)(((uint64_t)w.x << 21) | (uint64_t)(w.y >> 11)) * (1.0 / 9007199254740992.0);
+  int step = 0;
+  if (step < n_steps - 1 && !(cdf0 > u)) ++step;
+  if (step == 1 && step < n_steps - 1 && !(cdf1 > u)) ++step;
+  int64_t cur = seeds_q[i];
+  cur = cur < 0 ? 0 : (cur >= n_nodes ? n_nodes - 1 : cur);
+  for (int h = 1; h <= step; ++h) {
+    const int64_t beg = indptr[cur];
+    const uint32_t deg = (uint32_t)(indptr[cur + 1] - beg);
+    if (deg == 0u) break;
+    const u32x4 r = philox_at(key, sample, 0, (uint32_t)h, 0, GCCB_TAG_KHOP);
+    cur = indices[beg + __umulhi(r.y, deg)];
+  }
+  seeds_k[i] = cur;
+}
+
 }  // namespace gccb
 
 using namespace gccb;
@@ -584,7 +790,7 @@ extern "C" int gccb_sample_batch(const gccb_graph_t* graph, const int64_t* seeds
   const long long want_cap = 2ll * (long long)batch->edge_cap;
   const int pool_cap = (int)(want_cap < 0x7fff0000ll ? want_cap : 0x7fff0000ll);
   cudaMemsetAsync(pool_counter, 0, sizeof(unsigned long long), (cudaStream_t)stream);
-  auto k1 = rwr_walk_unique_kernel;
+  auto k1 = rwr_walk_unique_kernel<kModeRwr>;
   auto k3 = induce_fill_kernel;
   if (smem > 48 * 1024) {
     gccb::ensure_dyn_smem(k1, smem);
@@ -592,7 +798,8 @@ extern "C" int gccb_sample_batch(const gccb_graph_t* graph, const int64_t* seeds
   }
   GCCB_LAUNCH(k1, 2 * B, GCCB_ST, smem, stream, graph->indptr, graph->indices, graph->n_nodes, graph->budget_table,
               graph->budget_table_len, graph->restart_thresh, graph->key, seeds, sample_ids, B,
-              cap_n, subv, subdeg, rowstart, pool, pool_cap, pool_counter, batch->counters, batch->flags);
+              cap_n, subv, subdeg, rowstart, pool, pool_cap, pool_counter, batch->counters, batch->flags,
+              (const int64_t*)nullptr, 0, 0, 0);
   GCCB_LAUNCH(batch_offsets_kernel, 2, 256, 0, stream, batch->counters, B, batch->node_cap,
               batch->edge_cap, batch->node_off, batch->edge_off, batch->flags);
   GCCB_LAUNCH(k3, 2 * B, GCCB_ST, smem, stream, graph->indptr, graph->indices, batch->counters, B,
@@ -600,4 +807,133 @@ extern "C" int gccb_sample_batch(const gccb_graph_t* graph, const int64_t* seeds
               batch->edge_off, batch->indptr, batch->indices, batch->sub_deg, batch->graph_id,
               batch->orig_id);
   return check_launch("gccb_sample_batch");
+}
+
+// ---- the reference's other views: k-hop key seeds (step_dist) and neighbour sampling (aug="ns") ----------------
+
+extern "C" int gccb_pair_seeds(const gccb_graph_t* graph, const double* step_cdf, int32_t n_steps,
+                               const int64_t* seeds_q, const int64_t* sample_ids, int32_t count, int64_t* seeds_k,
+                               gccb_stream_t stream) {
+  if (!graph || !graph->indptr || !graph->indices || graph->n_nodes <= 0 || !step_cdf || n_steps < 1 ||
+      n_steps > 3 || !seeds_q || !sample_ids || !seeds_k || count < 0) {
+    set_last_error("gccb_pair_seeds: bad argument");
+    return GCCB_ERR_BADARG;
+  }
+  if (count == 0) return GCCB_OK;
+  GCCB_LAUNCH(pair_seeds_kernel, (count + 127) / 128, 128, 0, stream, graph->indptr, graph->indices, graph->n_nodes,
+              graph->key, step_cdf[0], n_steps > 1 ? step_cdf[1] : 1.0, (int)n_steps, seeds_q, sample_ids, (int)count,
+              seeds_k);
+  return check_launch("pair_seeds_kernel");
+}
+
+extern "C" int gccb_sample_batch_pairs(const gccb_graph_t* graph, const int64_t* seeds_q, const int64_t* seeds_k,
+                                       const int64_t* sample_ids, const gccb_batch_t* batch, void* workspace,
+                                       size_t workspace_bytes, gccb_stream_t stream) {
+  if (!graph || !batch || !seeds_q || !seeds_k || !sample_ids || !workspace || batch->batch <= 0 ||
+      graph->max_budget <= 0 || !graph->indptr || !graph->indices || !graph->budget_table) {
+    set_last_error("gccb_sample_batch_pairs: bad argument");
+    return GCCB_ERR_BADARG;
+  }
+  const int B = batch->batch;
+  const int cap_n = sampler_cap_n(graph->max_budget);
+  if (workspace_bytes < gccb_sample_batch_workspace(B, graph->max_budget, batch->edge_cap)) {
+    set_last_error("gccb_sample_batch_pairs: workspace too small");
+    return GCCB_ERR_CAPACITY;
+  }
+  const int P = pow2_ge(graph->max_budget + (int)GCCB_HOPCAP);
+  const size_t smem = (size_t)P * sizeof(int);
+  if (smem > 200 * 1024) {
+    set_last_error("gccb_sample_batch_pairs: walk budget %d needs %zu B of shared memory (> 200 KiB)",
+                   graph->max_budget, smem);
+    return GCCB_ERR_CAPACITY;
+  }
+  int32_t* subv = (int32_t*)workspace;
+  int32_t* subdeg = subv + (size_t)2 * B * cap_n;
+  int32_t* rowstart = subdeg + (size_t)2 * B * cap_n;
+  unsigned long long* pool_counter = (unsigned long long*)(rowstart + (size_t)2 * B * cap_n);
+  int32_t* pool = (int32_t*)pool_counter + 16;
+  const long long want_cap = 2ll * (long long)batch->edge_cap;
+  const int pool_cap = (int)(want_cap < 0x7fff0000ll ? want_cap : 0x7fff0000ll);
+  cudaMemsetAsync(pool_counter, 0, sizeof(unsigned long long), (cudaStream_t)stream);
+  auto k1 = rwr_walk_unique_kernel<kModePairs>;
+  auto k3 = induce_fill_kernel;
+  if (smem > 48 * 1024) {
+    gccb::ensure_dyn_smem(k1, smem);
+    gccb::ensure_dyn_smem(k3, smem);
+  }
+  GCCB_LAUNCH(k1, 2 * B, GCCB_ST, smem, stream, graph->indptr, graph->indices, graph->n_nodes, graph->budget_table,
+              graph->budget_table_len, graph->restart_thresh, graph->key, seeds_q, sample_ids, B,
+              cap_n, subv, subdeg, rowstart, pool, pool_cap, pool_counter, batch->counters, batch->flags,
+              seeds_k, 0, 0, 0);
+  GCCB_LAUNCH(batch_offsets_kernel, 2, 256, 0, stream, batch->counters, B, batch->node_cap,
+              batch->edge_cap, batch->node_off, batch->edge_off, batch->flags);
+  GCCB_LAUNCH(k3, 2 * B, GCCB_ST, smem, stream, graph->indptr, graph->indices, batch->counters, B,
+              cap_n, batch->node_cap, batch->edge_cap, subv, subdeg, rowstart, pool, batch->node_off,
+              batch->edge_off, batch->indptr, batch->indices, batch->sub_deg, batch->graph_id,
+              batch->orig_id);
+  return check_launch("gccb_sample_batch_pairs");
+}
+
+// shared memory of an ns ego-net of cap vertices: V[cap] | F[cap] | S[pow2 >= max(k, 2) * cap]
+static size_t ns_smem(int cap, int k) { return (size_t)4 * (2 * (size_t)cap + (size_t)pow2_ge((k < 2 ? 2 : k) * cap)); }
+#define GCCB_NS_SMEM (192 * 1024)
+// An ego-net over its cap is counted node_cap + 1 vertices, so that batch_offsets_kernel publishes its view empty.
+// That kernel sums the counts of 256 samples in an int block scan: 256 * (node_cap + 1) must stay below 2^31.
+#define GCCB_NS_NODE_CAP_MAX (0x7fffffff / 256 - 1)
+
+extern "C" int32_t gccb_ns_ego_cap(int32_t num_neighbors) {
+  if (num_neighbors < 1 || num_neighbors > 0xffff) return 0;
+  for (int cap = 65536; cap >= 64; cap >>= 1)
+    if ((long long)num_neighbors * cap <= (1 << 24) && ns_smem(cap, num_neighbors) <= GCCB_NS_SMEM) return cap;
+  return 0;
+}
+
+extern "C" size_t gccb_ns_batch_workspace(int32_t batch, int32_t num_neighbors, int32_t edge_cap) {
+  const int cap = gccb_ns_ego_cap(num_neighbors);
+  return ((size_t)3 * (size_t)(2 * batch) * (size_t)cap + 16 + (size_t)2 * (size_t)edge_cap) * sizeof(int32_t);
+}
+
+extern "C" int gccb_ns_batch(const gccb_graph_t* graph, const int64_t* seeds_q, const int64_t* seeds_k,
+                             const int64_t* sample_ids, int32_t num_hops, int32_t num_neighbors,
+                             const gccb_batch_t* batch, void* workspace, size_t workspace_bytes,
+                             gccb_stream_t stream) {
+  const int cap = gccb_ns_ego_cap(num_neighbors);
+  if (!graph || !batch || !seeds_q || !seeds_k || !sample_ids || !workspace || batch->batch <= 0 ||
+      !graph->indptr || !graph->indices || graph->n_nodes <= 0 || num_hops < 0 || num_hops > 0xffff || cap == 0) {
+    set_last_error("gccb_ns_batch: bad argument (num_hops 0..65535, num_neighbors 1..%d)", 0xffff);
+    return GCCB_ERR_BADARG;
+  }
+  if (batch->node_cap > GCCB_NS_NODE_CAP_MAX) {
+    set_last_error("gccb_ns_batch: node_cap %d above %d", batch->node_cap, GCCB_NS_NODE_CAP_MAX);
+    return GCCB_ERR_CAPACITY;
+  }
+  const int B = batch->batch;
+  if (workspace_bytes < gccb_ns_batch_workspace(B, num_neighbors, batch->edge_cap)) {
+    set_last_error("gccb_ns_batch: workspace too small");
+    return GCCB_ERR_CAPACITY;
+  }
+  const size_t smem1 = ns_smem(cap, num_neighbors), smem3 = (size_t)cap * sizeof(int);
+  int32_t* subv = (int32_t*)workspace;
+  int32_t* subdeg = subv + (size_t)2 * B * cap;
+  int32_t* rowstart = subdeg + (size_t)2 * B * cap;
+  unsigned long long* pool_counter = (unsigned long long*)(rowstart + (size_t)2 * B * cap);
+  int32_t* pool = (int32_t*)pool_counter + 16;
+  const long long want_cap = 2ll * (long long)batch->edge_cap;
+  const int pool_cap = (int)(want_cap < 0x7fff0000ll ? want_cap : 0x7fff0000ll);
+  cudaMemsetAsync(pool_counter, 0, sizeof(unsigned long long), (cudaStream_t)stream);
+  auto k1 = rwr_walk_unique_kernel<kModeNs>;
+  auto k3 = induce_fill_kernel;
+  if (smem1 > 48 * 1024) gccb::ensure_dyn_smem(k1, smem1);
+  if (smem3 > 48 * 1024) gccb::ensure_dyn_smem(k3, smem3);
+  GCCB_LAUNCH(k1, 2 * B, GCCB_ST, smem1, stream, graph->indptr, graph->indices, graph->n_nodes,
+              (const int32_t*)nullptr, 0, 0u, graph->key, seeds_q, sample_ids, B, cap, subv, subdeg, rowstart, pool,
+              pool_cap, pool_counter, batch->counters, batch->flags, seeds_k, (int)num_hops, (int)num_neighbors,
+              batch->node_cap);
+  GCCB_LAUNCH(batch_offsets_kernel, 2, 256, 0, stream, batch->counters, B, batch->node_cap,
+              batch->edge_cap, batch->node_off, batch->edge_off, batch->flags);
+  GCCB_LAUNCH(k3, 2 * B, GCCB_ST, smem3, stream, graph->indptr, graph->indices, batch->counters, B,
+              cap, batch->node_cap, batch->edge_cap, subv, subdeg, rowstart, pool, batch->node_off,
+              batch->edge_off, batch->indptr, batch->indices, batch->sub_deg, batch->graph_id,
+              batch->orig_id);
+  return check_launch("gccb_ns_batch");
 }

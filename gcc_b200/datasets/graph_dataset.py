@@ -8,6 +8,8 @@ positional features and batching all run as CUDA kernels over a CSR kept in HBM:
   reference (CPU worker processes)                      here (device kernels)
   __iter__: np.random.choice(p ~ deg^.75)   :85-92   -> gccb_draw_seeds
   __getitem__: budget + dgl RWR             :113-130 -> gccb_sample_batch (walk)
+    step_dist key seed, dgl random_walk     :104-110 -> gccb_pair_seeds, then gccb_sample_batch_pairs
+    aug="ns" neighbour sampling             :131-162 -> gccb_ns_batch
   _rwr_trace_to_dgl_graph                   data_util.py:218-239 -> gccb_sample_batch (induce)
   _add_undirected_graph_positional_embedding data_util.py:266-281 -> gccb_posenc
   batcher()/dgl.batch, pickling, H2D        data_util.py:26-32, train.py:382-383 -> (nothing: already batched on device)
@@ -28,6 +30,7 @@ from . import synthetic
 from .data_util import BatchedSubgraphs
 
 HOPCAP = 64
+NS_NODE_CAP_MAX = (2 ** 31 - 1) // 256 - 1   # gccb_ns_batch: an ego-net over its cap counts node_cap + 1 vertices
 
 
 def load_graphs(spec):
@@ -123,6 +126,7 @@ class BatchBuffers:
         self.pos = torch.zeros(2, node_cap, pos_dim, dtype=torch.float32, device=device)
         self.eigvals = torch.zeros(2 * B, pos_dim, dtype=torch.float32, device=device)
         self.seeds = torch.zeros(B, dtype=torch.int64, device=device)
+        self.seeds_k = torch.zeros(B, dtype=torch.int64, device=device)      # key-view seeds of step_dist
         self.sample_ids = torch.zeros(B, dtype=torch.int64, device=device)
         ws = lib.gccb_sample_batch_workspace(B, max_budget, edge_cap) if max_budget is not None else 0
         self.ws_sample = torch.zeros(max(ws, 8), dtype=torch.uint8, device=device)
@@ -152,7 +156,7 @@ class BatchBuffers:
             s.edge_off = self.edge_off.view(-1)[:2 * (b + 1)].view(2, b + 1)
             s.counters = self.counters[:2 * b]
             s.eigvals = self.eigvals[:2 * b]
-            s.seeds, s.sample_ids = self.seeds[:b], self.sample_ids[:b]
+            s.seeds, s.seeds_k, s.sample_ids = self.seeds[:b], self.seeds_k[:b], self.sample_ids[:b]
             s.c = s._batch_struct()
             self._narrowed[b] = s
         return self._narrowed[b]
@@ -187,10 +191,55 @@ class BatchBuffers:
                     n for b, n in _capi.FLAG_NAMES.items() if f & b))
 
 
+def step_cdf(step_dist):
+    """float64 CDF of step_dist (the number of hops between the q and k seeds, graph_dataset.py:104-110), or None
+    for the default [1, 0, 0] (both views share the seed).  Lengths 1 to 3, as the reference's random_walk allows."""
+    p = [float(x) for x in step_dist]
+    if not 1 <= len(p) <= 3 or min(p) < 0.0 or abs(sum(p) - 1.0) > 1e-9:
+        raise ValueError("step_dist must hold 1 to 3 probabilities summing to 1, got %r" % (step_dist,))
+    if p[0] == 1.0:
+        return None
+    cdf = np.cumsum(np.array(p, dtype=np.float64))
+    return np.ascontiguousarray(cdf / cdf[-1])
+
+
+def sample_views(ds, buf, st):
+    """Both views of buf's B pairs from buf.seeds / buf.sample_ids, as `ds` asks: its step_cdf (None: the k view
+    shares the seed; else gccb_pair_seeds draws buf.seeds_k on the device) and its aug ("rwr": gccb_sample_batch, or
+    gccb_sample_batch_pairs for separate seeds; "ns": gccb_ns_batch).  No host sync."""
+    lib = _lib.get()
+    g = ds.graph
+    cdf, aug = getattr(ds, "step_cdf", None), getattr(ds, "aug", "rwr")   # the labeled datasets: the defaults
+    seeds_k = buf.seeds
+    if cdf is not None:
+        _lib.check(lib.gccb_pair_seeds(C.byref(g.c), cdf.ctypes.data, len(cdf), _lib.dptr(buf.seeds),
+                                       _lib.dptr(buf.sample_ids), buf.B, _lib.dptr(buf.seeds_k), st),
+                   "gccb_pair_seeds")
+        seeds_k = buf.seeds_k
+    ws = (_lib.dptr(buf.ws_sample), buf.ws_sample.numel(), st)
+    if aug == "ns":
+        _lib.check(lib.gccb_ns_batch(C.byref(g.c), _lib.dptr(buf.seeds), _lib.dptr(seeds_k), _lib.dptr(buf.sample_ids),
+                                     ds.rw_hops, ds.num_neighbors, C.byref(buf.c), *ws), "gccb_ns_batch")
+    elif seeds_k is buf.seeds:
+        _lib.check(lib.gccb_sample_batch(C.byref(g.c), _lib.dptr(buf.seeds), _lib.dptr(buf.sample_ids),
+                                         C.byref(buf.c), *ws), "gccb_sample_batch")
+    else:
+        _lib.check(lib.gccb_sample_batch_pairs(C.byref(g.c), _lib.dptr(buf.seeds), _lib.dptr(seeds_k),
+                                               _lib.dptr(buf.sample_ids), C.byref(buf.c), *ws),
+                   "gccb_sample_batch_pairs")
+
+
 class LoadBalanceGraphDataset(torch.utils.data.IterableDataset):
     """Same constructor as the reference (graph_dataset.py:34-47) plus `device`, `seed`,
     `batch_size` and capacity knobs.  `dgl_graphs_file` may be a CSRGraph, a list of
-    CSRGraphs or an .npz path."""
+    CSRGraphs or an .npz path.
+
+    step_dist = [p0, p1, p2]: the k view's seed is the end of a 0-, 1- or 2-hop uniform walk from the q seed, drawn
+    per sample on the device; both views keep the q seed's walk budget (graph_dataset.py:104-130).  aug="ns" replaces
+    RWR by neighbour sampling: rw_hops layers, each expanding the previous one by at most num_neighbors neighbours
+    per vertex (:131-162).  With the reference's default rw_hops (train.py: 256) that reaches most of a component;
+    an ego-net holds at most gccb_ns_ego_cap(num_neighbors) vertices (4096 at num_neighbors = 5) and a view at most
+    node_cap, and a view that does not fit is skipped like any overflowing batch."""
 
     def __init__(self, rw_hops=64, restart_prob=0.8, positional_embedding_size=32,
                  step_dist=[1.0, 0.0, 0.0], num_workers=1, dgl_graphs_file="./data/small.bin",
@@ -199,16 +248,17 @@ class LoadBalanceGraphDataset(torch.utils.data.IterableDataset):
         super(LoadBalanceGraphDataset).__init__()
         assert sum(step_dist) == 1.0
         assert positional_embedding_size > 1
-        if list(step_dist) != [1.0, 0.0, 0.0]:
-            raise NotImplementedError("only the default step_dist=[1,0,0] (q and k share the seed, "
-                                      "graph_dataset.py:39,104-106) is on the accelerated path")
-        if aug != "rwr":
-            raise NotImplementedError("aug='ns' is not on the accelerated path (train.py never sets it)")
+        self.step_cdf = step_cdf(step_dist)
+        if aug not in ("rwr", "ns"):
+            raise NotImplementedError("aug=%r: the reference defines 'rwr' and 'ns'" % (aug,))
+        if aug == "ns" and int(num_neighbors) < 1:
+            raise ValueError("aug='ns' needs num_neighbors >= 1")
         if graph_transform is not None:
-            raise NotImplementedError("graph_transform is unused by train.py and unsupported here")
+            raise NotImplementedError("graph_transform is an arbitrary callable on DGLGraphs: it cannot run on the "
+                                      "device and is unsupported here")
         self.rw_hops, self.restart_prob = rw_hops, restart_prob
         self.positional_embedding_size = positional_embedding_size
-        self.step_dist, self.num_samples, self.num_neighbors = step_dist, num_samples, num_neighbors
+        self.step_dist, self.num_samples, self.num_neighbors = step_dist, num_samples, int(num_neighbors)
         self.dgl_graphs_file, self.aug, self.graph_transform = dgl_graphs_file, aug, graph_transform
         graph, graph_sizes = load_graphs(dgl_graphs_file)
         # the reference's greedy size-descending worker balance (graph_dataset.py:63-76); kept for
@@ -233,6 +283,15 @@ class LoadBalanceGraphDataset(torch.utils.data.IterableDataset):
         mb = self.graph.max_budget
         self.node_cap = int(node_cap or (B * min(mb + HOPCAP, 320) + mb + HOPCAP))
         self.edge_cap = int(edge_cap or self.node_cap * 16)
+        if aug == "ns":
+            # the ns workspace holds ego-nets of up to ego_cap vertices: sizing the buffers' sampler workspace as for
+            # that walk budget gives every copy of them (PretrainEngine's run-ahead ring) room for it
+            ego_cap = int(_lib.get().gccb_ns_ego_cap(self.num_neighbors))
+            if ego_cap == 0:
+                raise ValueError("num_neighbors=%d is too large for aug='ns'" % self.num_neighbors)
+            if self.node_cap > NS_NODE_CAP_MAX:
+                raise ValueError("aug='ns' takes node_cap <= %d, got %d" % (NS_NODE_CAP_MAX, self.node_cap))
+            mb = max(mb, ego_cap)
         self.buffers = BatchBuffers(B, self.node_cap, self.edge_cap, positional_embedding_size, mb,
                                     self.device)
         self.next_sample = 0
@@ -258,10 +317,7 @@ class LoadBalanceGraphDataset(torch.utils.data.IterableDataset):
         else:
             buf.seeds.copy_(seeds, non_blocking=True)
             buf.sample_ids.copy_(torch.arange(first_sample, first_sample + B, device=self.device))
-        _lib.check(lib.gccb_sample_batch(C.byref(self.graph.c), _lib.dptr(buf.seeds),
-                                         _lib.dptr(buf.sample_ids), C.byref(buf.c),
-                                         _lib.dptr(buf.ws_sample), buf.ws_sample.numel(), st),
-                   "gccb_sample_batch")
+        sample_views(self, buf, st)
         if posenc:
             self.posenc(buf)
         return buf
@@ -307,8 +363,9 @@ class _EpochOrder:
 class NodeClassificationDataset(_EpochOrder):
     """generate.py's dataset (graph_dataset.py:279-309 on top of GraphDataset :218-275): item idx is
     NODE idx of one graph, seeds are taken in order (no sampling), both views walk from the seed
-    (step_dist [1,0,0]) with budget max(rw_hops, int(deg*e/(e-1)/restart + 0.5)) -- plain degree,
-    unlike the pretraining loader.  `dataset` is a CSRGraph or an .npz path (the reference's
+    (step_dist [1,0,0]; another step_dist walks the k view from a 1- or 2-hop neighbour, graph_dataset.py:227-275)
+    with budget max(rw_hops, int(deg*e/(e-1)/restart + 0.5)) of the q seed -- plain degree, unlike the pretraining
+    loader.  `dataset` is a CSRGraph or an .npz path (the reference's
     downloaded datasets need the network / DGL).  Iterating yields batched (graph_q, graph_k, count)
     with `count` valid pairs (the last batch is padded with the last node).  sample_batch() is the
     pretraining interface (see _EpochOrder)."""
@@ -317,8 +374,8 @@ class NodeClassificationDataset(_EpochOrder):
                  positional_embedding_size=32, step_dist=[1.0, 0.0, 0.0], device="cuda", seed=0,
                  batch_size=256, node_cap=None, edge_cap=None):
         assert positional_embedding_size > 1
-        if list(step_dist) != [1.0, 0.0, 0.0]:
-            raise NotImplementedError("only step_dist=[1,0,0] (generate.py never sets another)")
+        self.step_cdf = step_cdf(step_dist)
+        self.aug, self.num_neighbors = "rwr", 5
         self.rw_hops, self.subgraph_size, self.restart_prob = rw_hops, subgraph_size, restart_prob
         self.positional_embedding_size, self.step_dist = positional_embedding_size, step_dist
         graph, _ = load_graphs(dataset)
@@ -354,13 +411,10 @@ class NodeClassificationDataset(_EpochOrder):
             raise ValueError("a node dataset trains on its nodes in order: the seeds are not the caller's")
         epoch, a, b = self._locate(first_sample)
         buf = (buffers or self.buffers).narrow(b)
-        lib = _lib.get()
         torch.arange(a, a + b, device=self.device, out=buf.seeds)
         base = epoch * self.total
         torch.arange(base + a, base + a + b, device=self.device, out=buf.sample_ids)
-        _lib.check(lib.gccb_sample_batch(C.byref(self.graph.c), _lib.dptr(buf.seeds), _lib.dptr(buf.sample_ids),
-                                         C.byref(buf.c), _lib.dptr(buf.ws_sample), buf.ws_sample.numel(),
-                                         _lib.stream_ptr()), "gccb_sample_batch")
+        sample_views(self, buf, _lib.stream_ptr())
         if posenc:
             self.posenc(buf)
         return buf
@@ -396,6 +450,9 @@ class GraphClassificationDataset(_EpochOrder):
                  step_dist=[1.0, 0.0, 0.0], device="cuda", seed=0, batch_size=32):
         from . import downstream
         assert positional_embedding_size > 1
+        if step_cdf(step_dist) is not None:
+            raise NotImplementedError("step_dist other than [1,0,0] on whole graphs would need the k view relabelled "
+                                      "seed first around another vertex, per view and batch; unsupported")
         self.rw_hops, self.subgraph_size, self.restart_prob = rw_hops, subgraph_size, restart_prob
         self.positional_embedding_size, self.step_dist = positional_embedding_size, step_dist
         self.entire_graph = True

@@ -112,6 +112,37 @@ int gccb_sample_batch(const gccb_graph_t* graph, const int64_t* seeds,
                       const int64_t* sample_ids, const gccb_batch_t* batch, void* workspace,
                       size_t workspace_bytes, gccb_stream_t stream);
 
+/* Key seeds of step_dist (graph_dataset.py:104-110).  Sample i (Philox sample id sample_ids[i]) draws
+ * step = first index with step_cdf > u (u: 53 Philox bits, tag GCCB_TAG_STEP; step_cdf: n_steps <= 3 host
+ * doubles, read at the call, last = 1) and writes in seeds_k[i] the end of a `step`-hop uniform walk from
+ * seeds_q[i] (hop h drawn with tag GCCB_TAG_KHOP, hop field h); a vertex without neighbours ends the walk.
+ * One thread per sample, no workspace, no host sync.                                                      */
+int gccb_pair_seeds(const gccb_graph_t* graph, const double* step_cdf, int32_t n_steps, const int64_t* seeds_q,
+                    const int64_t* sample_ids, int32_t count, int64_t* seeds_k, gccb_stream_t stream);
+
+/* gccb_sample_batch with separate view seeds (graph_dataset.py:113-130 with step > 0): view 0 walks from
+ * and induces around seeds_q[i], view 1 around seeds_k[i] (its row 0); BOTH walk budgets come from
+ * seeds_q[i]'s degree.  Workspace: gccb_sample_batch_workspace.                                            */
+int gccb_sample_batch_pairs(const gccb_graph_t* graph, const int64_t* seeds_q, const int64_t* seeds_k,
+                            const int64_t* sample_ids, const gccb_batch_t* batch, void* workspace,
+                            size_t workspace_bytes, gccb_stream_t stream);
+
+/* Neighbour-sampled ego-nets (aug="ns", graph_dataset.py:131-162).  View 0 from seeds_q[i], view 1 from
+ * seeds_k[i] (pass seeds_q twice for step_dist [1,0,0]).  Layer 0 = {seed}; layer h = the de-duplicated
+ * union over the vertices u of layer h-1 of all neighbour entries of u if deg(u) <= num_neighbors, else
+ * num_neighbors distinct entries drawn uniformly without replacement, for num_hops layers (early stop when a
+ * layer is empty or the union is closed under neighbourhood).  Node set = [seed, union minus seed ascending],
+ * then the same induced sub-CSR, sub_deg, graph_id, orig_id and flags as gccb_sample_batch; counters =
+ * (n, m, layers expanded, sum of parent degrees).  An ego-net holds at most gccb_ns_ego_cap(num_neighbors)
+ * vertices (shared memory: 4096 at num_neighbors = 5); a larger one, like a view over node_cap / edge_cap,
+ * raises GCCB_FLAG_NODE_OVERFLOW and its view is published empty.  node_cap <= 2^31 / 256 - 2.  The graph's
+ * budget table and restart threshold are not read.                                                        */
+int32_t gccb_ns_ego_cap(int32_t num_neighbors);
+size_t gccb_ns_batch_workspace(int32_t batch, int32_t num_neighbors, int32_t edge_cap);
+int gccb_ns_batch(const gccb_graph_t* graph, const int64_t* seeds_q, const int64_t* seeds_k,
+                  const int64_t* sample_ids, int32_t num_hops, int32_t num_neighbors, const gccb_batch_t* batch,
+                  void* workspace, size_t workspace_bytes, gccb_stream_t stream);
+
 /* Whole-graph batches (entire_graph=True, graph_dataset.py:311-340; dgl.batch, data_util.py:26-32).
  * A set of graphs as one union CSR: graph i owns vertices node_off[i] .. node_off[i+1) and entries
  * edge_off[i] .. edge_off[i+1) (= indptr[node_off[i]] ..), rows as listed (parallel edges, self loops and
