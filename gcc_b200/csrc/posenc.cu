@@ -7,28 +7,23 @@
 // k <= 0 -> zeros.  The reference runs ARPACK (scipy eigsh, float64, random v0)
 // per ego-net on a CPU worker: ~2.8 ms each, the dominant cost of its pipeline.
 //
-// Three device solvers, one CTA (or one cluster) per ego-net, chosen by size through device-built work lists:
+// Two device solvers, one CTA (or one cluster) per ego-net, chosen by size through device-built work lists:
 //
-//  (0) n <= 96 by default (up to 228 with GCCB200_DENSE_MAX): the dense tridiagonal solver -- Householder
+//  (0) n <= 96 (up to 228 with GCCB200_DENSE_MAX): the dense tridiagonal solver -- Householder
 //      tridiagonalisation of the whole matrix in shared memory, multisection on Sturm counts, inverse iteration
 //      with one common shift per multiple eigenvalue, Gram-Schmidt inside clusters, back-transformation in
 //      registers.  A direct method: eigenvalues / residuals / orthonormality to 1e-6.  See its own comment below.
+//      Three classes: n <= 96, 144 and 228 (the last two only when GCCB200_DENSE_MAX reaches them).
 //
-//  (1) n <= 64, only with solver (0) off: dense one-sided (Hestenes) Jacobi.  G = L + 2I (SPD, spectrum in [1,3]) lives in
-//      shared memory, column-major; plane rotations applied on the right orthogonalise its
-//      columns; because G is symmetric positive definite the converged columns are
-//      lambda_j' v_j, so the eigenvectors are the normalised columns and no V matrix is stored.
-//      A warp owns one column pair per step of a round-robin tournament; dot products by
-//      shuffle reduction, rotations in registers.
-//
-//  (2) every larger n: Chebyshev-filtered subspace iteration (ChFSI) on a block of 48 vectors, any n.
-//      Ego-nets are star-like: their spectra have one huge degenerate cluster, so a degree-4/8
-//      Chebyshev filter on [-1, cut] followed by Rayleigh-Ritz converges in ~3 outer iterations
-//      (measured on the C2 workload).  Per iteration: 8 sparse products with the sub-CSR (fused
-//      three-term recurrence), CGS2 re-orthonormalisation, H = Q^T L Q, the 48x48 Ritz problem
-//      solved by solver (1) in shared memory, X = Q W, residual check.  The n x 48 blocks live in
-//      an L2-resident workspace (2 blocks per ego-net), so shared memory does not bound n and
-//      8 CTAs fit per SM.  Cost is O(n * 48^2) instead of the O(n^3) of a dense solve.
+//  (1) every larger n: Chebyshev-filtered subspace iteration (ChFSI) on a block of 48 vectors, any n.
+//      Ego-nets are star-like: their spectra have one huge degenerate cluster, so a Chebyshev filter on
+//      [-1, cut] followed by Rayleigh-Ritz converges in ~3 outer iterations (measured on the C2 workload).
+//      Per iteration: up to 16 sparse products with the sub-CSR (fused three-term recurrence), panel
+//      Gram-Schmidt, H = Q^T L Q, the 48x48 Ritz problem by two-sided Jacobi (jacobi_ritz48) in shared
+//      memory, X = Q W, residual check.  Cost is O(n * 48^2) instead of the O(n^3) of a dense solve.
+//      Where the two n x 48 blocks live depends on n: in the shared memory of one CTA for n <= 160 and
+//      n <= 384, spread over the shared memory of a cluster of 8 CTAs for n <= 1536 and n <= 3584, in an
+//      L2-resident workspace above that.
 //
 // All return an orthonormal basis of every eigenspace (degenerate clusters included), Ritz
 // values as Rayleigh quotients, a deterministic sign (largest-|.| component positive) and are
@@ -39,9 +34,7 @@
 
 namespace gccb {
 
-#define GCCB_EIG_SMALL 64          // largest n solved by the dense Jacobi kernel
-#define GCCB_EIG_MAXSWEEP 14
-#define GCCB_EIG_TOL 1.0e-6f
+#define GCCB_EIG_MAXSWEEP 14       // Jacobi sweeps of a Ritz solve
 #define GCCB_CF_B 48               // ChFSI block size (>= pos_dim 32 + guard vectors)
 // Chebyshev degree per outer iteration: as high as the fp32 block tolerates.  The filter on [-1, cut] gains
 // T_d(x1), x1 = (3 - cut) / (1 + cut), on the top eigenvalue relative to the damped interval; directions whose
@@ -78,19 +71,14 @@ namespace gccb {
 #ifndef GCCB_CF_SWEEPS0_CLUSTER
 #define GCCB_CF_SWEEPS0_CLUSTER 1
 #endif
-#define GCCB_CF_NSM_A 96            // shared-memory block classes: n <= 96 (3 CTAs/SM) and
-#define GCCB_CF_NSM 160            //   n <= 160 (2 CTAs/SM),
+#define GCCB_DN_A 96               // dense solver classes: n <= 96 (always dense), n <= 144, n <= 228
+#define GCCB_DN_B 144
+#define GCCB_DN_C 228
+#define GCCB_CF_NSM 160            // ChFSI shared-memory block classes: n <= 160 (2 CTAs/SM),
 #define GCCB_CF_NSM_C 384          //   n <= 384 (one GCCB_BIG_NT-thread CTA; 150 KB + 30 KB static leave room
                                    //   for a 46 KB training CTA on the same SM);
 #define GCCB_CF_NSM_D1 1536        //   n <= 1536: cluster of 8 CTAs (DSMEM), 192-row slabs (75 KB per CTA);
 #define GCCB_CF_NSM_D 3584         //   n <= 3584: cluster of 8 CTAs, 448-row slabs; larger: L2 workspace
-#define GCCB_EIG_NCLASS 7
-#ifndef GCCB_CF_SMEM_PAD_A
-#define GCCB_CF_SMEM_PAD_A 0       // A/B builds: extra shared memory per n <= 96 CTA (lowers its CTAs per SM)
-#endif
-#ifndef GCCB_CAP_MID1
-#define GCCB_CAP_MID1 (GCCB_NUM_SMS * 3)     // persistent grid of the n <= 96 class (3 CTAs per SM)
-#endif
 #ifndef GCCB_CAP_MID2
 #define GCCB_CAP_MID2 (GCCB_NUM_SMS * 2)     // persistent grid of the n <= 160 class (2 CTAs per SM)
 #endif
@@ -121,131 +109,39 @@ namespace gccb {
 #endif
 #define GCCB_TICK(k) do { if (threadIdx.x == 0) { long long t_ = GCCB_CLK(); ph[k] += t_ - t_last; t_last = t_; } } while (0)
 
-// class 0: n <= 64 (dense Jacobi); 1, 2, 3: ChFSI with shared-memory blocks; 4, 5: ChFSI on a cluster;
-// 6: ChFSI with L2 blocks
-__device__ __forceinline__ int eig_class(int n) {
-  return n <= GCCB_EIG_SMALL ? 0 : n <= GCCB_CF_NSM_A ? 1 : n <= GCCB_CF_NSM ? 2 : n <= GCCB_CF_NSM_C ? 3 :
-         n <= GCCB_CF_NSM_D1 ? 4 : n <= GCCB_CF_NSM_D ? 5 : 6;
+// Size classes: 0, 1, 2: dense solver (n <= 96 / 144 / 228, the last two up to dense_max only); 3, 4: ChFSI with
+// shared-memory blocks (n <= 160 / 384); 5, 6: ChFSI on a cluster (n <= 1536 / 3584); 7: ChFSI with L2 blocks
+#define GCCB_EIG_NCLASS 8
+__device__ __forceinline__ int eig_class(int n, int dense_max) {
+  if (n <= dense_max) return n <= GCCB_DN_A ? 0 : n <= GCCB_DN_B ? 1 : 2;
+  return n <= GCCB_CF_NSM ? 3 : n <= GCCB_CF_NSM_C ? 4 : n <= GCCB_CF_NSM_D1 ? 5 : n <= GCCB_CF_NSM_D ? 6 : 7;
 }
 
-// Work lists: worklist[c][i] = slot.  One CTA, deterministic order.  grid = 1, block = 256.
-// Ego-nets up to `dense_max` vertices go to the dense tridiagonal solver instead (lists dense_list[3][2B], classes
-// n <= dn_a / dn_b / larger; dense_max = 0: none).
+// Work lists: worklist[c][i] = slot, counts[c] entries per class.  One CTA, deterministic order.  grid = 1,
+// block = 256.
 __global__ void __launch_bounds__(256)
 posenc_classify_kernel(const int64_t* __restrict__ counters, const int32_t* __restrict__ node_off,
-                       int B, int32_t* __restrict__ worklist, int32_t* __restrict__ counts,
-                       int dense_max, int dn_a, int dn_b, int32_t* __restrict__ dense_list,
-                       int32_t* __restrict__ dense_counts) {
+                       int B, int dense_max, int32_t* __restrict__ worklist, int32_t* __restrict__ counts) {
   __shared__ int scan_scratch[33];
   const int tid = threadIdx.x;
-  constexpr int NC = GCCB_EIG_NCLASS + 3;
-  int base[NC] = {0};
+  int base[GCCB_EIG_NCLASS] = {0};
   for (int s0 = 0; s0 < 2 * B; s0 += 256) {
     int slot = s0 + tid;
     int cls = -1;
     if (slot < 2 * B) {
       int view = slot / B;
-      if (node_off[view * (B + 1) + B] >= 0) {
-        const int n = (int)counters[(size_t)slot * 4];
-        cls = n <= dense_max ? GCCB_EIG_NCLASS + (n <= dn_a ? 0 : n <= dn_b ? 1 : 2) : eig_class(n);
-      }
+      if (node_off[view * (B + 1) + B] >= 0) cls = eig_class((int)counters[(size_t)slot * 4], dense_max);
     }
 #pragma unroll
-    for (int c = 0; c < NC; ++c) {
+    for (int c = 0; c < GCCB_EIG_NCLASS; ++c) {
       int tot;
       int ex = block_scan_excl(cls == c ? 1 : 0, scan_scratch, &tot);
-      if (cls == c) {
-        if (c < GCCB_EIG_NCLASS) worklist[(size_t)c * 2 * B + base[c] + ex] = slot;
-        else dense_list[(size_t)(c - GCCB_EIG_NCLASS) * 2 * B + base[c] + ex] = slot;
-      }
+      if (cls == c) worklist[(size_t)c * 2 * B + base[c] + ex] = slot;
       base[c] += tot;
     }
   }
   if (tid < GCCB_EIG_NCLASS) counts[tid] = base[tid];
-  if (tid < 3) dense_counts[tid] = base[GCCB_EIG_NCLASS + tid];
 }
-
-// ------------------------------------------------------------------------------------------------
-// One-sided Jacobi on the n x n column-major matrix G (leading dimension ld) in shared memory:
-// orthogonalises the columns in place; on return nrm[j] = ||g_j||.  Returns the number of
-// sweeps used (== GCCB_EIG_MAXSWEEP means not converged).  NR = ceil(nmax/32) rows per lane.
-template <int NR, int THREADS>
-__device__ __forceinline__ int jacobi_onesided(float* G, float* nrm, int n, int ld) {
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  constexpr int NW = THREADS / 32;
-  const int m = n + (n & 1);                            // tournament size (even)
-  int sweep = 0;
-  for (; sweep < GCCB_EIG_MAXSWEEP; ++sweep) {
-    for (int p = warp; p < n; p += NW) {                // exact column norms once per sweep
-      float s = 0.f;
-#pragma unroll
-      for (int jj = 0; jj < NR; ++jj) {
-        int r = lane + 32 * jj;
-        float x = r < n ? G[(size_t)p * ld + r] : 0.f;
-        s = fmaf(x, x, s);
-      }
-      s = warp_sum(s);
-      if (lane == 0) nrm[p] = s;
-    }
-    __syncthreads();
-    int rotated = 0;
-    for (int r = 0; r < m - 1; ++r) {
-      for (int pi = warp; pi < m / 2; pi += NW) {
-        int p, q;
-        if (pi == 0) { p = m - 1; q = r; }
-        else { p = (r + pi) % (m - 1); q = (r + m - 1 - pi) % (m - 1); }
-        if (p >= n || q >= n) continue;                 // bye (odd n)
-        if (p > q) { int t = p; p = q; q = t; }
-        float gp[NR], gq[NR];
-        float gam = 0.f;
-#pragma unroll
-        for (int jj = 0; jj < NR; ++jj) {
-          int rr = lane + 32 * jj;
-          gp[jj] = rr < n ? G[(size_t)p * ld + rr] : 0.f;
-          gq[jj] = rr < n ? G[(size_t)q * ld + rr] : 0.f;
-          gam = fmaf(gp[jj], gq[jj], gam);
-        }
-        // read the cached norms BEFORE the shuffle reduction: the shuffles are the
-        // convergence point that orders these reads against lane 0's update below
-        const float alpha = nrm[p], beta = nrm[q];
-        gam = warp_sum(gam);
-        if (fabsf(gam) > GCCB_EIG_TOL * sqrtf(alpha * beta)) {      // warp-uniform
-          const float zeta = (beta - alpha) / (2.0f * gam);
-          const float t = (zeta >= 0.f ? 1.0f : -1.0f) / (fabsf(zeta) + sqrtf(1.0f + zeta * zeta));
-          const float c = 1.0f / sqrtf(1.0f + t * t);
-          const float s = c * t;
-#pragma unroll
-          for (int jj = 0; jj < NR; ++jj) {
-            int rr = lane + 32 * jj;
-            if (rr < n) {
-              G[(size_t)p * ld + rr] = c * gp[jj] - s * gq[jj];
-              G[(size_t)q * ld + rr] = s * gp[jj] + c * gq[jj];
-            }
-          }
-          if (lane == 0) { nrm[p] = alpha - t * gam; nrm[q] = beta + t * gam; }
-          rotated = 1;
-        }
-      }
-      __syncthreads();
-    }
-    if (!__syncthreads_or(rotated)) break;
-  }
-  for (int p = warp; p < n; p += NW) {                  // final norms: nrm[j] = ||g_j||
-    float s = 0.f;
-#pragma unroll
-    for (int jj = 0; jj < NR; ++jj) {
-      int r = lane + 32 * jj;
-      float x = r < n ? G[(size_t)p * ld + r] : 0.f;
-      s = fmaf(x, x, s);
-    }
-    s = warp_sum(s);
-    if (lane == 0) nrm[p] = sqrtf(s);
-  }
-  __syncthreads();
-  return sweep;
-}
-
-
 
 // Two-sided Jacobi specialised for the even-order Ritz problem (m = 48): per round ONE thread per pair
 // derives (c, s); then every thread applies BOTH sides of the similarity transform to whole 2 x 2
@@ -411,114 +307,7 @@ __device__ __forceinline__ void write_features(int n, int k, int pos_dim, int no
   }
 }
 
-// ---- solver (1): dense one-sided Jacobi, n <= 64 ---------------------------------------------------
-// (one-sided on the SPD matrix L + 2I keeps eigenVECTOR accuracy for close eigenvalues -- paths,
-// rings -- where an fp32 two-sided rotation sequence loses it as eps * rotations / gap; fp64 would
-// too be accurate but runs at a small fraction of the fp32 rate on this part)
-__device__ __forceinline__ void posenc_jacobi_item(const int item, const int32_t* __restrict__ worklist, const int32_t* __restrict__ counts,
-                     int B, int node_cap, int edge_cap, const int32_t* __restrict__ node_off,
-                     const int32_t* __restrict__ b_indptr, const int32_t* __restrict__ b_indices,
-                     const int32_t* __restrict__ sub_deg, int pos_dim, int normalize,
-                     float* __restrict__ pos, float* __restrict__ eigvals, int32_t* __restrict__ flags,
-                     int32_t* __restrict__ dbg_iters, float* __restrict__ dbg_res) {
-  __shared__ float G[GCCB_EIG_SMALL * GCCB_EIG_SMALL];
-  __shared__ float nrm[GCCB_EIG_SMALL];
-  __shared__ float dinv[GCCB_EIG_SMALL];
-  __shared__ int sel[32];
-  __shared__ float sgn[32];
-  const int slot = worklist[item];
-  const int view = slot / B, g = slot - view * B;
-  const int noff = node_off[view * (B + 1) + g];
-  const int n = node_off[view * (B + 1) + g + 1] - noff;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int k = min(n - 2, pos_dim);
-  float* out = pos + ((size_t)view * node_cap + noff) * pos_dim;
-  if (k <= 0) {                                        // data_util.py:243-244
-    for (int i = tid; i < n * pos_dim; i += 256) out[i] = 0.f;
-    if (eigvals)
-      for (int i = tid; i < pos_dim; i += 256) eigvals[(size_t)slot * pos_dim + i] = 0.f;
-    return;
-  }
-  const int ld = n;
-  const int32_t* v_indptr = b_indptr + (size_t)view * (node_cap + 1);
-  const int32_t* v_indices = b_indices + (size_t)view * edge_cap;
-  const int32_t* v_deg = sub_deg + (size_t)view * node_cap;
-  for (int i = tid; i < n * ld; i += 256) G[i] = 0.f;
-  for (int i = tid; i < n; i += 256) {
-    int d = v_deg[noff + i];
-    dinv[i] = 1.0f / sqrtf((float)(d < 1 ? 1 : d));   // in_degrees().clip(1) ** -0.5
-  }
-  __syncthreads();
-  for (int i = warp; i < n; i += 8) {                  // row i <- its in-neighbours j
-    const int beg = v_indptr[noff + i], end = v_indptr[noff + i + 1];
-    const float di = dinv[i];
-    for (int e = beg + lane; e < end; e += 32) {
-      int j = v_indices[e] - noff;
-      atomicAdd(&G[(size_t)j * ld + i], di * dinv[j]);  // shared-memory adds of exact products
-    }
-  }
-  __syncthreads();
-  for (int i = tid; i < n; i += 256) G[(size_t)i * ld + i] += 2.0f;
-  __syncthreads();
-  const int sweeps = jacobi_onesided<2, 256>(G, nrm, n, ld);
-  if (sweeps == GCCB_EIG_MAXSWEEP && tid == 0) atomicOr(flags, (int)GCCB_FLAG_EIG_NOCONV);
-  if (tid == 0) { dbg_iters[slot] = -sweeps; dbg_res[slot] = 0.f; }
-  // eigenvalue of column j = ||g_j|| - 2; rank columns, keep the k largest, ascending
-  const float* mu = nrm;
-  for (int j = tid; j < n; j += 256) {
-    const float mj = mu[j];
-    int rank = 0;
-    for (int i = 0; i < n; ++i) {
-      float mi = mu[i];
-      rank += (mi > mj) || (mi == mj && i < j);
-    }
-    if (rank < k) sel[k - 1 - rank] = j;                // ascending: slot k-1 = largest
-  }
-  __syncthreads();
-  if (eigvals) {
-    // eigenvalues as Rayleigh quotients v^T L v against the ORIGINAL sparse matrix: the column
-    // norms carry the accumulated rounding of ~n rotations per sweep (~1e-5)
-    for (int c = warp; c < pos_dim; c += 8) {
-      float acc = 0.f;
-      if (c < k) {
-        const float* col = G + (size_t)sel[c] * ld;
-        for (int i = lane; i < n; i += 32) {
-          const int beg = v_indptr[noff + i], end = v_indptr[noff + i + 1];
-          float rowacc = 0.f;
-          for (int e = beg; e < end; ++e) {
-            int j = v_indices[e] - noff;
-            rowacc = fmaf(dinv[j], col[j], rowacc);
-          }
-          acc = fmaf(col[i] * dinv[i], rowacc, acc);
-        }
-        acc = warp_sum(acc);
-        const float m2 = mu[sel[c]];
-        acc = acc / (m2 * m2);
-      }
-      if (lane == 0) eigvals[(size_t)slot * pos_dim + c] = acc;
-    }
-  }
-  const float* Gc = G;
-  const int* selc = sel;
-  write_features(n, k, pos_dim, normalize, sgn, out,
-                 [&](int c, int r) { const int j = selc[c]; return Gc[(size_t)j * ld + r] / mu[j]; });
-}
-
-__global__ void __launch_bounds__(256)
-posenc_jacobi_kernel(const int32_t* __restrict__ worklist, const int32_t* __restrict__ counts,
-                     int B, int node_cap, int edge_cap, const int32_t* __restrict__ node_off,
-                     const int32_t* __restrict__ b_indptr, const int32_t* __restrict__ b_indices,
-                     const int32_t* __restrict__ sub_deg, int pos_dim, int normalize,
-                     float* __restrict__ pos, float* __restrict__ eigvals, int32_t* __restrict__ flags,
-                     int32_t* __restrict__ dbg_iters, float* __restrict__ dbg_res) {
-  // persistent over the work list: the grid is sized for the typical count, not for 2B
-  for (int item = blockIdx.x; item < counts[0]; item += gridDim.x) {
-    posenc_jacobi_item(item, worklist, counts, B, node_cap, edge_cap, node_off, b_indptr, b_indices, sub_deg, pos_dim, normalize, pos, eigvals, flags, dbg_iters, dbg_res);
-    __syncthreads();
-  }
-}
-
-// ---- solver (2): Chebyshev-filtered subspace iteration, any n > 64 -------------------------------
+// ---- solver (1): Chebyshev-filtered subspace iteration, any n > 96 -------------------------------
 // Blocks are ROW-major n x 48 (leading dimension ld): a neighbour gather reads one contiguous row,
 // so the sparse products are warp-per-row with lanes across the 48 columns (any degree, coalesced).
 struct SubCsr {
@@ -645,7 +434,7 @@ __device__ __forceinline__ void posenc_chfsi_item(const int item, const int32_t*
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   constexpr int NW = NT / 32;
   const bool hi = lane < CB - 32;
-  const int k = min(n - 2, pos_dim);                    // n > 64 -> k = pos_dim
+  const int k = min(n - 2, pos_dim);                    // n > 96 -> k = pos_dim
   float* out = pos + ((size_t)view * node_cap + noff) * pos_dim;
   float* dinv = dinv_g + (size_t)view * node_cap + noff;
   SubCsr S;
@@ -674,7 +463,6 @@ __device__ __forceinline__ void posenc_chfsi_item(const int item, const int32_t*
     X[(size_t)(i / CB) * ld + (i % CB)] = (float)(int32_t)w.x * (1.0f / 2147483648.0f);
   }
   __syncthreads();
-#ifndef GCCB_CF_NO_DEFLATE
   // The top eigenvector of D^-1/2 A D^-1/2 is known in closed form: v0 = sqrt(deg) (eigenvalue 1; ||v0||^2 =
   // sum of degrees).  It becomes column 0 and is projected out of the random columns: the first filter
   // amplifies the v0 component ~35x more than anything below 0.5, so without this every filtered column is
@@ -691,7 +479,6 @@ __device__ __forceinline__ void posenc_chfsi_item(const int item, const int32_t*
     }
     __syncthreads();
   }
-#endif
   float cut = 0.0f;                                     // the filter suppresses [-1, cut]
   float prev_worst = 3.0e38f;
   bool converged = false;
@@ -821,11 +608,7 @@ __device__ __forceinline__ void posenc_chfsi_item(const int item, const int32_t*
             const bool tiny = !(g[0] > 1e-30f) || !(g[2] > 1e-30f) || !(g[5] > 1e-30f) || !(g[9] > 1e-30f);
             const bool again = !(g[0] > 0.5f * yy0) || !(g[2] > 0.5f * yy1) || !(g[5] > 0.5f * yy2) || !(g[9] > 0.5f * yy3);
             float li[10] = {1.f, 0.f, 1.f, 0.f, 0.f, 1.f, 0.f, 0.f, 0.f, 1.f};   // identity: projection only
-#ifdef GCCB_GS_FORCE_SCALAR                              // A/B builds (profiles/build_variant.py)
-            if (true) flag = 2;
-#else
             if (tiny) flag = 2;
-#endif
             else if (again) flag = pass == 0 ? 1 : 2;
             else {
               const float l00 = sqrtf(g[0]);
@@ -1051,7 +834,7 @@ posenc_chfsi_kernel(const int32_t* __restrict__ worklist, const int32_t* __restr
 }
 
 
-// ---- solver (3): ChFSI over a thread-block cluster (distributed shared memory), n > 480 ------------
+// ---- solver (1) on a thread-block cluster (distributed shared memory), 384 < n <= 3584 -------------
 // A hub ego-net (up to ~3400 vertices at the C2 walk budget) would otherwise keep ONE SM busy for
 // tens of milliseconds while 147 idle.  Here a cluster of CS CTAs owns it: rows are partitioned,
 // each CTA keeps its slice of both n x 48 blocks in its own shared memory, neighbour rows are
@@ -1559,9 +1342,6 @@ posenc_chfsi_cluster_kernel(const int32_t* __restrict__ worklist, const int32_t*
 //   6. a residual check against the sparse matrix (reported per ego-net; NOCONV above GCCB_DN_RES_FLAG).
 //
 // Z (n x 32) lives in the dead upper-right corner of the matrix (rows < n - 32, columns >= n - 32) plus a 32 x 32 tail.
-#define GCCB_DN_A 96
-#define GCCB_DN_B 144
-#define GCCB_DN_C 228
 #ifndef GCCB_DN_INVIT
 #define GCCB_DN_INVIT 3
 #endif
@@ -1591,7 +1371,7 @@ __device__ __forceinline__ int dn_sturm(const float* __restrict__ d, const float
   return c;
 }
 
-template <int NMAX, int NT, bool USM>
+template <int NMAX, int NT>
 __device__ __forceinline__ void posenc_dense_item(const int slot, int B, int node_cap, int edge_cap,
                     const int32_t* __restrict__ node_off, const int32_t* __restrict__ b_indptr,
                     const int32_t* __restrict__ b_indices, const int32_t* __restrict__ sub_deg, int pos_dim, int normalize,
@@ -1614,7 +1394,6 @@ __device__ __forceinline__ void posenc_dense_item(const int slot, int B, int nod
   __shared__ float lam[32], lamp[32], lo[32], hi[32], sgn[32];
   __shared__ int cnt[NT];
   __shared__ float part[NW * 32];
-  __shared__ float ufac[USM ? 2 * 32 * NMAX : 1];        // factor rows of the inverse iteration (USM: else in L2)
   long long ph[8] = {0, 0, 0, 0, 0, 0, 0, 0}, t_last = GCCB_CLK();
   const int view = slot / B, g = slot - view * B;
   const int noff = node_off[view * (B + 1) + g];
@@ -1636,8 +1415,8 @@ __device__ __forceinline__ void posenc_dense_item(const int slot, int B, int nod
   const int32_t* v_indices = b_indices + (size_t)view * edge_cap;
   const int32_t* v_deg = sub_deg + (size_t)view * node_cap;
   // factor rows of the inverse iteration: two n x 32 arrays in this ego-net's part of the L2 workspace
-  float* U0 = USM ? ufac : blocks + ((size_t)view * node_cap + noff) * (GCCB_CF_B + 1);
-  float* U1 = USM ? ufac + 32 * NMAX : U0 + (size_t)2 * node_cap * (GCCB_CF_B + 1);
+  float* U0 = blocks + ((size_t)view * node_cap + noff) * (GCCB_CF_B + 1);
+  float* U1 = U0 + (size_t)2 * node_cap * (GCCB_CF_B + 1);
   // ---- the matrix ---------------------------------------------------------------------------------------------
   for (int i = tid; i < NP; i += NT) { d[i] = 0.f; e[i] = 0.f; e2[i] = 0.f; taus[i] = 0.f; vbuf[i] = 0.f; pbuf[i] = 0.f; xbuf[i] = 0.f; }
   for (int i = tid; i < n; i += NT) {
@@ -2075,7 +1854,7 @@ __device__ __forceinline__ void posenc_dense_item(const int slot, int B, int nod
   write_features(n, k, pos_dim, normalize, sgn, out, [&](int c, int r_) { return zrow(r_)[c]; });
 }
 
-template <int NMAX, int NT, bool USM>
+template <int NMAX, int NT>
 __global__ void __launch_bounds__(NT, 65536 / 64 / NT)
 posenc_dense_kernel(const int32_t* __restrict__ worklist /* this class */, const int32_t* __restrict__ count,
                     int B, int node_cap, int edge_cap, const int32_t* __restrict__ node_off,
@@ -2084,7 +1863,7 @@ posenc_dense_kernel(const int32_t* __restrict__ worklist /* this class */, const
                     float* __restrict__ pos, float* __restrict__ eigvals, int32_t* __restrict__ flags,
                     int32_t* __restrict__ dbg_iters, float* __restrict__ dbg_res, long long* __restrict__ dbg_phase) {
   for (int item = blockIdx.x; item < count[0]; item += gridDim.x) {
-    posenc_dense_item<NMAX, NT, USM>(worklist[item], B, node_cap, edge_cap, node_off, b_indptr, b_indices, sub_deg, pos_dim,
+    posenc_dense_item<NMAX, NT>(worklist[item], B, node_cap, edge_cap, node_off, b_indptr, b_indices, sub_deg, pos_dim,
                                 normalize, blocks, pos, eigvals, flags, dbg_iters, dbg_res, dbg_phase);
     __syncthreads();
   }
@@ -2094,27 +1873,27 @@ posenc_dense_kernel(const int32_t* __restrict__ worklist /* this class */, const
 
 using namespace gccb;
 
-// workspace: worklist[7][2B] | counts[7] | iters[2B] (ints) | pad | res[2B] | dinv[2*node_cap] | blocks[2][2*node_cap*49] (floats)
-static size_t posenc_ws_ints(int B) {
-  return (((size_t)GCCB_EIG_NCLASS * 2 * B + GCCB_EIG_NCLASS + 2 * B) + 63) & ~(size_t)63;
+// workspace: the debug area phase[2B][8] (cycle counters) | iters[2B] | res[2B], then worklist[NCLASS][2B] |
+// counts[NCLASS] | pad to 256 bytes | dinv[2*node_cap] | blocks[2][2*node_cap*49] (floats)
+static size_t posenc_ws_head(int B) {
+  const size_t bytes = (size_t)2 * B * (8 * sizeof(long long) + sizeof(int32_t) + sizeof(float)) +
+                       ((size_t)GCCB_EIG_NCLASS * 2 * B + GCCB_EIG_NCLASS) * sizeof(int32_t);
+  return (bytes + 255) & ~(size_t)255;
 }
 
 extern "C" size_t gccb_posenc_workspace(int32_t batch, int32_t node_cap) {
-  return posenc_ws_ints(batch) * sizeof(int32_t) +
-         ((size_t)2 * batch + (size_t)2 * node_cap + (size_t)2 * 2 * node_cap * (GCCB_CF_B + 1)) * sizeof(float) +
-         (size_t)2 * batch * 8 * sizeof(long long) + 64 +
-         ((size_t)3 * 2 * batch + 4) * sizeof(int32_t);        // work lists + counts of the dense solver (tail)
+  return posenc_ws_head(batch) + ((size_t)2 * node_cap + (size_t)2 * 2 * node_cap * (GCCB_CF_B + 1)) * sizeof(float);
 }
 
-// Largest ego-net handed to the dense tridiagonal solver.  Default: its first class, n <= 96 -- the larger classes
+// Largest ego-net handed to the dense tridiagonal solver: GCCB_DN_A = 96 by default, GCCB200_DENSE_MAX moves it up
+// to GCCB_DN_C = 228 (a smaller value behaves as 96).  The default stops at the first dense class: the larger ones
 // hold 108 / 224 KB of shared memory and 512 threads x 64 registers per CTA and crowd the training kernels that run
-// beside them in the pipeline out of their SMs.  GCCB200_DENSE_MAX overrides (0 = ChFSI / Jacobi for every size, 228 = direct-method accuracy
-// for every ego-net up to 228 vertices); read on every call so that a test can compare the solvers in one process.
+// beside them in the pipeline out of their SMs, so they are an accuracy option.  Read on every call so that a test
+// can compare settings in one process.
 static int posenc_dense_max() {
   const char* e = getenv("GCCB200_DENSE_MAX");
-  int v = GCCB_DN_A;
-  if (e && e[0]) v = atoi(e);
-  return v < 0 ? 0 : v > GCCB_DN_C ? GCCB_DN_C : v;
+  const int v = e && e[0] ? atoi(e) : GCCB_DN_A;
+  return v < GCCB_DN_A ? GCCB_DN_A : v > GCCB_DN_C ? GCCB_DN_C : v;
 }
 
 extern "C" int gccb_posenc(const gccb_batch_t* batch, int32_t pos_dim, int32_t normalize,
@@ -2124,24 +1903,25 @@ extern "C" int gccb_posenc(const gccb_batch_t* batch, int32_t pos_dim, int32_t n
     set_last_error("gccb_posenc: bad argument (pos_dim must be in [2, 32])");
     return GCCB_ERR_BADARG;
   }
+  if ((uintptr_t)workspace % sizeof(long long)) {
+    set_last_error("gccb_posenc: workspace must be 8-byte aligned");
+    return GCCB_ERR_BADARG;
+  }
   const int B = batch->batch;
   if (workspace_bytes < gccb_posenc_workspace(B, batch->node_cap)) {
     set_last_error("gccb_posenc: workspace too small");
     return GCCB_ERR_CAPACITY;
   }
-  int32_t* worklist = (int32_t*)workspace;
+  long long* dbg_phase = (long long*)workspace;                        // per slot: phase cycle counters
+  int32_t* dbg_iters = (int32_t*)(dbg_phase + (size_t)2 * B * 8);     // per slot: ChFSI outer iterations (dense: 0)
+  float* dbg_res = (float*)(dbg_iters + (size_t)2 * B);                // per slot: final residual
+  int32_t* worklist = (int32_t*)(dbg_res + (size_t)2 * B);
   int32_t* counts = worklist + (size_t)GCCB_EIG_NCLASS * 2 * B;
-  int32_t* dbg_iters = counts + GCCB_EIG_NCLASS;                       // per slot: ChFSI outer iterations (Jacobi: -sweeps)
-  float* dbg_res = (float*)((int32_t*)workspace + posenc_ws_ints(B));      // per slot: final residual
-  float* dinv = dbg_res + (size_t)2 * B;
+  float* dinv = (float*)((char*)workspace + posenc_ws_head(B));
   float* blocks = dinv + (size_t)2 * batch->node_cap;
-  // diagnostics tail: per-slot phase cycle counters (8-byte aligned)
-  long long* dbg_phase = (long long*)(((uintptr_t)(blocks + (size_t)2 * 2 * batch->node_cap * (GCCB_CF_B + 1)) + 15) & ~(uintptr_t)15);
-  int32_t* dense_list = (int32_t*)(dbg_phase + (size_t)2 * B * 8);
-  int32_t* dense_counts = dense_list + (size_t)3 * 2 * B;
   const int dense_max = posenc_dense_max();
-  GCCB_LAUNCH(posenc_classify_kernel, 1, 256, 0, stream, batch->counters, batch->node_off, B, worklist, counts,
-              dense_max, GCCB_DN_A, GCCB_DN_B, dense_list, dense_counts);
+  GCCB_LAUNCH(posenc_classify_kernel, 1, 256, 0, stream, batch->counters, batch->node_off, B, dense_max, worklist,
+              counts);
   auto kgiant = posenc_chfsi_kernel<0, 1024>;
 #ifndef GCCB_EMU
   constexpr int CLUSTER = 8;
@@ -2151,15 +1931,22 @@ extern "C" int gccb_posenc(const gccb_batch_t* batch, int32_t pos_dim, int32_t n
   auto khuge = posenc_chfsi_cluster_kernel<GCCB_BIG_NT, CLUSTER>;
   auto kbig = posenc_chfsi_kernel<1, GCCB_BIG_NT>;
   auto kmid = posenc_chfsi_kernel<1, 256>;
-  auto ksmall = posenc_jacobi_kernel;
-  const size_t s_a = (size_t)2 * GCCB_CF_NSM_A * (GCCB_CF_B + 1) * sizeof(float) + GCCB_CF_SMEM_PAD_A;
+  auto kd_a = posenc_dense_kernel<GCCB_DN_A, 256>;
+  auto kd_b = posenc_dense_kernel<GCCB_DN_B, 512>;
+  auto kd_c = posenc_dense_kernel<GCCB_DN_C, 512>;
   const size_t s_b = (size_t)2 * GCCB_CF_NSM * (GCCB_CF_B + 1) * sizeof(float);
   const size_t s_c = (size_t)2 * GCCB_CF_NSM_C * (GCCB_CF_B + 1) * sizeof(float);
   const size_t s_d = (size_t)2 * ((GCCB_CF_NSM_D + CLUSTER - 1) / CLUSTER) * (GCCB_CF_B + 1) * sizeof(float);
   const size_t s_d1 = (size_t)2 * ((GCCB_CF_NSM_D1 + CLUSTER - 1) / CLUSTER) * (GCCB_CF_B + 1) * sizeof(float);
+  const size_t sd_a = (size_t)GCCB_DN_A * dn_ld(GCCB_DN_A) * sizeof(float);
+  const size_t sd_b = (size_t)GCCB_DN_B * dn_ld(GCCB_DN_B) * sizeof(float);
+  const size_t sd_c = (size_t)GCCB_DN_C * dn_ld(GCCB_DN_C) * sizeof(float);
   gccb::ensure_dyn_smem(kmid, s_b);
   gccb::ensure_dyn_smem(kbig, s_c);
   gccb::ensure_dyn_smem(khuge, s_d);
+  gccb::ensure_dyn_smem(kd_a, sd_a);
+  gccb::ensure_dyn_smem(kd_b, sd_b);
+  gccb::ensure_dyn_smem(kd_c, sd_c);
   // The size classes are independent: fork them over side streams (event fork/join, legal inside
   // CUDA-graph capture) so that the few long-running large ego-nets overlap the many small ones.
 #ifndef GCCB_EMU
@@ -2171,10 +1958,10 @@ extern "C" int gccb_posenc(const gccb_batch_t* batch, int32_t pos_dim, int32_t n
   cudaEvent_t* ev_join = kit->ev;
   cudaStream_t main_s = (cudaStream_t)stream;
   cudaEventRecord(ev_fork, main_s);
-  for (int i = 0; i < 5; ++i) cudaStreamWaitEvent(side[i], ev_fork, 0);
-  gccb_stream_t s_giant = side[4], s_huge = side[0], s_big = side[1], s_mid2 = side[2], s_small = side[3], s_mid1 = stream;
+  for (int i = 0; i < 4; ++i) cudaStreamWaitEvent(side[i], ev_fork, 0);
+  gccb_stream_t s_giant = side[3], s_huge = side[0], s_big = side[1], s_mid = side[2];
 #else
-  gccb_stream_t s_giant = stream, s_huge = stream, s_big = stream, s_mid2 = stream, s_small = stream, s_mid1 = stream;
+  gccb_stream_t s_giant = stream, s_huge = stream, s_big = stream, s_mid = stream;
 #endif
 #define GCCB_PE_ARGS(cls) worklist, counts, cls, B, batch->node_cap, batch->edge_cap, batch->node_off, batch->indptr, \
     batch->indices, batch->sub_deg, pos_dim, normalize, blocks, dinv, pos, eigvals, batch->flags, dbg_iters, dbg_res, dbg_phase
@@ -2182,11 +1969,11 @@ extern "C" int gccb_posenc(const gccb_batch_t* batch, int32_t pos_dim, int32_t n
   // idle CTA of these kernels still has to win 1024 thread slots / up to 188 KB of shared memory
   // just to exit, which costs concurrent kernels dearly
   auto capped = [&](int limit) { return 2 * B < limit ? 2 * B : limit; };
-  GCCB_LAUNCH(kgiant, capped(8), 1024, 0, s_giant, GCCB_PE_ARGS(6));
-  // two cluster launches: 192-row slabs (class 4) and 448-row slabs (class 5, same stream as the
+  GCCB_LAUNCH(kgiant, capped(8), 1024, 0, s_giant, GCCB_PE_ARGS(7));
+  // two cluster launches: 192-row slabs (class 5) and 448-row slabs (class 6, same stream as the
   // L2 fallback: both are rare); persistent over their work lists
   for (int pass = 0; pass < 2; ++pass) {
-    const int cls = pass == 0 ? 4 : 5;
+    const int cls = pass == 0 ? 5 : 6;
     const size_t smem = pass == 0 ? s_d1 : s_d;
     const int items = capped(pass == 0 ? 8 : 4);
     gccb_stream_t st = pass == 0 ? s_huge : s_giant;
@@ -2209,47 +1996,22 @@ extern "C" int gccb_posenc(const gccb_batch_t* batch, int32_t pos_dim, int32_t n
                 eigvals, batch->flags, dbg_iters, dbg_res, dbg_phase);
 #endif
   }
-  if (dense_max > 0) {
-    // dense classes: n <= 96 (256 threads, 48 KB: four CTAs per SM), n <= 144 (512 threads, 108 KB: two per SM),
-    // n <= 228 (512 threads, 224 KB: one per SM); on the streams of the ChFSI classes they replace
-    // GCCB200_DN_USM=1: class A keeps the factor rows of the inverse iteration in shared memory (74 KB per CTA, three
-    // per SM) instead of the L2 workspace (50 KB, four per SM): a shorter inverse iteration for a larger footprint,
-    // off by default.
-    const char* usm_e = getenv("GCCB200_DN_USM");
-    const bool usm = usm_e && usm_e[0] == '1';
-    auto kd_a = usm ? posenc_dense_kernel<GCCB_DN_A, 256, true> : posenc_dense_kernel<GCCB_DN_A, 256, false>;
-    auto kd_b = posenc_dense_kernel<GCCB_DN_B, 512, false>;
-    auto kd_c = posenc_dense_kernel<GCCB_DN_C, 512, false>;
-    const size_t sd_a = (size_t)GCCB_DN_A * dn_ld(GCCB_DN_A) * sizeof(float);
-    const size_t sd_b = (size_t)GCCB_DN_B * dn_ld(GCCB_DN_B) * sizeof(float);
-    const size_t sd_c = (size_t)GCCB_DN_C * dn_ld(GCCB_DN_C) * sizeof(float);
-    gccb::ensure_dyn_smem(posenc_dense_kernel<GCCB_DN_A, 256, true>, sd_a);
-    gccb::ensure_dyn_smem(posenc_dense_kernel<GCCB_DN_A, 256, false>, sd_a);
-    gccb::ensure_dyn_smem(kd_b, sd_b);
-    gccb::ensure_dyn_smem(kd_c, sd_c);
-#define GCCB_DN_ARGS(c) dense_list + (size_t)(c) * 2 * B, dense_counts + (c), B, batch->node_cap, batch->edge_cap, \
+  // dense classes: n <= 96 (256 threads, 48 KB: four CTAs per SM), n <= 144 (512 threads, 108 KB: two per SM),
+  // n <= 228 (512 threads, 224 KB: one per SM); the first on the caller's stream, the others on the streams of the
+  // ChFSI classes they replace
+#define GCCB_DN_ARGS(c) worklist + (size_t)(c) * 2 * B, counts + (c), B, batch->node_cap, batch->edge_cap, \
     batch->node_off, batch->indptr, batch->indices, batch->sub_deg, pos_dim, normalize, blocks, pos, eigvals, \
     batch->flags, dbg_iters, dbg_res, dbg_phase
-    // (diagnostics: GCCB200_DN_CAP_A / _B / _C override the persistent grid sizes, i.e. the CTAs per SM)
-    auto env_cap = [](const char* name, int dflt) { const char* e = getenv(name); const int v = e && e[0] ? atoi(e) : dflt; return v > 0 ? v : dflt; };
-    // classes above dense_max have empty lists: not launched (an idle CTA of theirs must still win 108 / 224 KB of
-    // shared memory to exit -- 40-170 us at the head of the streams of the ChFSI classes, CUPTI timeline)
-    if (dense_max > GCCB_DN_B)
-      GCCB_LAUNCH(kd_c, capped(env_cap("GCCB200_DN_CAP_C", GCCB_CAP_DN_C)), 512, sd_c, s_big, GCCB_DN_ARGS(2));
-    if (dense_max > GCCB_DN_A)
-      GCCB_LAUNCH(kd_b, capped(env_cap("GCCB200_DN_CAP_B", GCCB_CAP_DN_B)), 512, sd_b, s_mid2, GCCB_DN_ARGS(1));
-    GCCB_LAUNCH(kd_a, capped(env_cap("GCCB200_DN_CAP_A", usm ? GCCB_NUM_SMS * 3 : GCCB_CAP_DN_A)), 256, sd_a, s_mid1, GCCB_DN_ARGS(0));
-  }
-  GCCB_LAUNCH(kbig, capped(GCCB_NUM_SMS), GCCB_BIG_NT, s_c, s_big, GCCB_PE_ARGS(3));
-  // classes the dense solver covers completely have empty lists: not launched
-  if (dense_max < GCCB_CF_NSM) GCCB_LAUNCH(kmid, capped(GCCB_CAP_MID2), 256, s_b, s_mid2, GCCB_PE_ARGS(2));
-  if (dense_max < GCCB_CF_NSM_A) GCCB_LAUNCH(kmid, capped(GCCB_CAP_MID1), 256, s_a, s_mid1, GCCB_PE_ARGS(1));
-  if (dense_max < GCCB_EIG_SMALL)
-    GCCB_LAUNCH(ksmall, capped(GCCB_NUM_SMS), 256, 0, s_small, worklist, counts, B, batch->node_cap, batch->edge_cap,
-                batch->node_off, batch->indptr, batch->indices, batch->sub_deg, pos_dim, normalize, pos, eigvals,
-                batch->flags, dbg_iters, dbg_res);
+  // classes above dense_max have empty lists: not launched (an idle CTA of theirs must still win 108 / 224 KB of
+  // shared memory to exit -- 40-170 us at the head of the streams of the ChFSI classes, CUPTI timeline)
+  if (dense_max > GCCB_DN_B) GCCB_LAUNCH(kd_c, capped(GCCB_CAP_DN_C), 512, sd_c, s_big, GCCB_DN_ARGS(2));
+  if (dense_max > GCCB_DN_A) GCCB_LAUNCH(kd_b, capped(GCCB_CAP_DN_B), 512, sd_b, s_mid, GCCB_DN_ARGS(1));
+  GCCB_LAUNCH(kd_a, capped(GCCB_CAP_DN_A), 256, sd_a, stream, GCCB_DN_ARGS(0));
+  GCCB_LAUNCH(kbig, capped(GCCB_NUM_SMS), GCCB_BIG_NT, s_c, s_big, GCCB_PE_ARGS(4));
+  // the n <= 160 class is empty when the dense solver covers it: not launched
+  if (dense_max < GCCB_CF_NSM) GCCB_LAUNCH(kmid, capped(GCCB_CAP_MID2), 256, s_b, s_mid, GCCB_PE_ARGS(3));
 #ifndef GCCB_EMU
-  for (int i = 0; i < 5; ++i) {
+  for (int i = 0; i < 4; ++i) {
     cudaEventRecord(ev_join[i], side[i]);
     cudaStreamWaitEvent(main_s, ev_join[i], 0);
   }

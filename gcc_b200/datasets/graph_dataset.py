@@ -163,14 +163,18 @@ class BatchBuffers:
 
     def eig_debug(self):
         """(iterations, worst residual) per ego-net of the last gccb_posenc on these buffers, read
-        from the debug area of its workspace (posenc.cu: worklist[7][2B] | counts[7] | iters[2B] |
-        pad to 64 ints | res[2B]).  Direct-Jacobi ego-nets report minus their sweep count, ego-nets solved by
-        the dense tridiagonal solver (a direct method) report 0 iterations and their measured residual."""
-        B, NC = self.B, 7
-        ints = self.ws_posenc.view(torch.int32)
-        o = NC * 2 * B + NC
-        ni = ((o + 2 * B + 63) // 64) * 64
-        return ints[o:o + 2 * B].clone(), self.ws_posenc[ni * 4: ni * 4 + 2 * B * 4].view(torch.float32).clone()
+        from the debug area at the start of its workspace (posenc.cu: phase[2B][8] int64 | iters[2B] int32 |
+        res[2B] float32).  Ego-nets solved by the dense tridiagonal solver (a direct method) report 0
+        iterations and their measured residual."""
+        n = 2 * self.B
+        ws = self.ws_posenc
+        return ws[64 * n:68 * n].view(torch.int32).clone(), ws[68 * n:72 * n].view(torch.float32).clone()
+
+    def eig_phases(self):
+        """[2B][8] int64 phase cycle counters per ego-net of the last gccb_posenc (thread 0 of each CTA, rank 0 of
+        each cluster), from the same debug area; posenc.cu names the phases of each solver."""
+        n = 2 * self.B
+        return self.ws_posenc[:64 * n].view(torch.int64).view(n, 8).clone()
 
     def check_flags(self):
         """Host sync: raise on any device-side failure flag.  Eigensolver non-convergence is not

@@ -174,8 +174,9 @@ int gccb_gather_graphs(const gccb_graph_set_t* set, const int64_t* graph_ids, co
  * Solvers by ego-net size (device-built work lists, csrc/posenc.cu): a dense tridiagonal
  * solver (Householder -> multisection -> inverse iteration; a direct method) for n <= 96,
  * Chebyshev-filtered subspace iteration above.  The environment variable
- * GCCB200_DENSE_MAX (0 .. 228, read on every call) moves that boundary: 0 = subspace
- * iteration / Jacobi for every size, 228 = direct-method accuracy up to 228 vertices.
+ * GCCB200_DENSE_MAX (96 .. 228, read on every call; smaller values act as 96) raises that
+ * boundary: 228 = direct-method accuracy up to 228 vertices.
+ * workspace: gccb_posenc_workspace(B, node_cap) bytes, 8-byte aligned.
  * Results are deterministic run to run for a given setting.                              */
 size_t gccb_posenc_workspace(int32_t batch, int32_t node_cap);
 int gccb_posenc(const gccb_batch_t* batch, int32_t pos_dim, int32_t normalize, float* pos,

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""GPU diagnostic: the dense tridiagonal eigensolver against the Jacobi / ChFSI classes on the same batches
+"""GPU diagnostic: the dense tridiagonal eigensolver up to 96 (the default) and up to 228 vertices on the same batches
 (gccb_posenc reads GCCB200_DENSE_MAX on every call), with the dense solver's phase cycle counters."""
 import ctypes as C
 import os
@@ -35,17 +35,7 @@ def posenc(buf, dense_max):
     return ev[0].elapsed_time(ev[1])
 
 
-def phases(buf):
-    ws = buf.ws_posenc
-    NC = 7
-    ni = (((NC * 2 * B + NC + 2 * B) + 63) // 64) * 64
-    cap = buf.node_cap
-    base = ws.data_ptr()
-    addr = (base + ni * 4 + (2 * B + 2 * cap + 2 * 2 * cap * 49) * 4 + 15) // 16 * 16
-    return ws[addr - base: addr - base + 2 * B * 8 * 8].view(torch.int64).view(2 * B, 8).cpu().numpy()
-
-
-variants = [("dense<=228", None), ("dense<=96", 96), ("iterative", 0)]
+variants = [("dense<=228", 228), ("dense<=96", None)]
 tot = {k: [] for k, _ in variants}
 for st in range(int(sys.argv[2]) if len(sys.argv) > 2 else 8):
     buf = ds.sample_batch(posenc=False)
@@ -59,13 +49,13 @@ for st in range(int(sys.argv[2]) if len(sys.argv) > 2 else 8):
     print("batch %d: largest n %s, flags %d, posenc ms %s" % (
         st, sorted(n.tolist())[-3:], flags, ", ".join("%s %.2f" % (k, tot[k][-1]) for k, _ in variants)))
 print("mean posenc ms per batch: " + ", ".join("%s %.3f" % (k, np.mean(v)) for k, v in tot.items()))
-posenc(buf, None)
+posenc(buf, 228)
 it, res = buf.eig_debug()
 it, res = it.cpu().numpy(), res.cpu().numpy()
-ph = phases(buf)
+ph = buf.eig_phases().cpu().numpy()
 n = buf.counters[:, 0].cpu().numpy()
 names = ["setup", "tridiagonalisation", "multisection", "inverse iteration", "gram-schmidt", "back-transformation"]
-for lo, hi in ((0, 64), (64, 96), (96, 144), (144, 228)):
+for lo, hi in ((0, 96), (96, 144), (144, 228)):
     m = (n > lo) & (n <= hi) & (it == 0)
     if m.sum():
         t = ph[m][:, :6].sum(0).astype(float)

@@ -28,15 +28,10 @@ for rep in range(3):
     ev[1].record()
     torch.cuda.synchronize()
     print("posenc ms", ev[0].elapsed_time(ev[1]))
-ws = buf.ws_posenc
-ints = ws.view(torch.int32)
-NC = 7
-ni = (((NC * 2 * B + NC + 2 * B) + 63) // 64) * 64
-iters = ints[NC * 2 * B + NC: NC * 2 * B + NC + 2 * B].cpu().numpy()
-res = ws[ni * 4: ni * 4 + 2 * B * 4].view(torch.float32).cpu().numpy()
+iters, res = (t.cpu().numpy() for t in buf.eig_debug())
 n = buf.counters[:, 0].cpu().numpy()
 print("flags", int(buf.flags.item()))
-for lo, hi in ((0, 64), (64, 96), (96, 160), (160, 480), (480, 1000), (1000, 100000)):
+for lo, hi in ((0, 96), (96, 160), (160, 384), (384, 1536), (1536, 100000)):
     m = (n > lo) & (n <= hi)
     if m.sum():
         print("n in (%d,%d]: count %d  iters mean %.2f max %d  res mean %.2e max %.2e" % (
@@ -53,24 +48,17 @@ for st in range(1, 9):
     ev[1].record()
     torch.cuda.synchronize()
     n = buf.counters[:, 0].cpu().numpy()
-    it = ints[NC * 2 * B + NC: NC * 2 * B + NC + 2 * B].cpu().numpy()
-    rs = ws[ni * 4: ni * 4 + 2 * B * 4].view(torch.float32).cpu().numpy()
+    it, rs = (t.cpu().numpy() for t in buf.eig_debug())
     top = np.argsort(-n)[:3]
     print("batch %d: posenc %.2f ms; largest (n, iters, res): %s; max iters %d" % (
         st, ev[0].elapsed_time(ev[1]), [(int(n[i]), int(it[i]), float("%.1e" % rs[i])) for i in top], it.max()))
 
-# phase cycle counters of the last batch (thread 0 of each CTA / rank 0 of each cluster)
-cap = buf.node_cap
-off_f = ni * 4 + (2 * B + 2 * cap + 2 * 2 * cap * 49) * 4
-off_f = (off_f + 15) // 16 * 16
-# the tail is aligned relative to the buffer base address
-base = ws.data_ptr()
-addr = (base + ni * 4 + (2 * B + 2 * cap + 2 * 2 * cap * 49) * 4 + 15) // 16 * 16
-phase = ws[addr - base: addr - base + 2 * B * 8 * 8].view(torch.int64).view(2 * B, 8).cpu().numpy()
+# phase cycle counters of the last batch's ChFSI ego-nets (thread 0 of each CTA / rank 0 of each cluster)
+phase = buf.eig_phases().cpu().numpy()
 names = ["filter", "gram-schmidt", "H=QtLQ", "ritz", "X=QW", "residual"]
 n = buf.counters[:, 0].cpu().numpy()
-for lo, hi in ((64, 96), (96, 160), (160, 480), (480, 100000)):
-    m = (n > lo) & (n <= hi)
+for lo, hi in ((96, 160), (160, 384), (384, 100000)):
+    m = (n > lo) & (n <= hi) & (it > 0)
     if m.sum():
         tot = phase[m][:, :6].sum(0).astype(float)
         print("n in (%d,%d]: cycles/ego-net %.0f k; split %s; Jacobi rounds/ego-net: %.0f working + %.0f idle" % (

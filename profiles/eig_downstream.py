@@ -4,7 +4,7 @@ eigensolver's inexactness do downstream?  VERDICT r01, missing #6.
 
 For one sampled batch (C2-like ego-nets, hubs included) the encoder (5-layer GIN, hidden 64, random init, train-mode
 BatchNorm, float64 oracle model) is run on positional features from
-  ours      the device solvers (emulated): default mix (dense n <= 96, ChFSI above), ChFSI only, dense up to 228;
+  ours      the device solvers (emulated): default mix (dense n <= 96, ChFSI above), dense up to 228;
   ours*     the SAME vectors projected onto the exact invariant subspace of the top-k eigenvalues (the whole multiple
             eigenvalue the cut falls into included) and re-orthonormalised (float64 eigh, polar factor): what the
             solver would return if it were exact, in the same basis -- so the difference
@@ -60,7 +60,7 @@ def main():
     laps = [opos.normalized_adjacency(s["indptr"], s["indices"], s["n"]).toarray() for s in lst]
     exact = [np.linalg.eigh(a) for a in laps]
     feats = {}
-    for name, dm in (("default (dense <= 96)", 96), ("ChFSI only", 0), ("dense <= 228", 228)):
+    for name, dm in (("default (dense <= 96)", 96), ("dense <= 228", 228)):
         b, pos = solver_features(views, dm)
         got, proj = [], []
         for gi, s in enumerate(lst):

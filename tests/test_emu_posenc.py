@@ -2,9 +2,9 @@
 spectral parity with the oracle (dense float64 eigh) and with the reference's own
 outputs (tests/golden/posenc_golden.npz).  Kernel LOGIC only; see test_gpu_*.
 
-Two solver families share the size range n <= 228: the dense tridiagonal solver (GCCB200_DENSE_MAX=228; the
-product default is 96) and the Jacobi / Chebyshev-filtered subspace iteration classes (GCCB200_DENSE_MAX=0); the
-variable is read by gccb_posenc on every call and the `solver` fixture runs every test through both."""
+The `solver` fixture runs a test through the shipped dispatch ("default": GCCB200_DENSE_MAX unset, the dense
+tridiagonal solver up to 96 vertices and the Chebyshev-filtered subspace iteration above) and through the dense
+solver up to 228 vertices ("dense": GCCB200_DENSE_MAX=228); gccb_posenc reads the variable on every call."""
 import ctypes as C
 import os
 
@@ -18,9 +18,12 @@ from oracle import posenc as opos
 G = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
-@pytest.fixture(params=["dense", "iterative"])
+@pytest.fixture(params=["default", "dense"])
 def solver(request, monkeypatch):
-    monkeypatch.setenv("GCCB200_DENSE_MAX", "0" if request.param == "iterative" else "228")
+    if request.param == "dense":
+        monkeypatch.setenv("GCCB200_DENSE_MAX", "228")
+    else:
+        monkeypatch.delenv("GCCB200_DENSE_MAX", raising=False)
     return request.param
 
 
@@ -40,6 +43,11 @@ def _posenc(views, normalize):
     return b, pos, eig
 
 
+def _views(graphs):
+    half = len(graphs) // 2
+    return [[_sub(g) for g in graphs[:half]], [_sub(g) for g in graphs[half:]]]
+
+
 def _check_spectral(sub, u, lam):
     n = sub["n"]
     k = min(n - 2, 32)
@@ -56,7 +64,7 @@ def _check_spectral(sub, u, lam):
     assert np.allclose(theta, w_exact, atol=1e-5)
 
 
-def test_jacobi_spectral_parity_small_and_degenerate(solver):
+def test_spectral_parity_small_and_degenerate(solver):
     graphs = [synthetic.path_graph(2), synthetic.path_graph(3), synthetic.path_graph(9),
               synthetic.star_graph(20), synthetic.triangle_tail(4),
               synthetic.erdos_renyi(40, 90, seed=1), synthetic.star_graph(50),
@@ -71,10 +79,10 @@ def test_jacobi_spectral_parity_small_and_degenerate(solver):
             _check_spectral(sub, pos[v, a:z], eig[v * b.B + gi])
 
 
-def test_jacobi_size_classes_and_normalisation(solver):
-    g1 = synthetic.erdos_renyi(90, 240, seed=7)           # 64 < n <= 96: Chebyshev-filtered subspace iteration
+def test_size_classes_and_normalisation(solver):
+    g1 = synthetic.erdos_renyi(90, 240, seed=7)           # n <= 96: dense solver
     g2 = synthetic.star_graph(90)                         # extreme degeneracy (eigenvalue 0 x 89)
-    g3 = synthetic.erdos_renyi(150, 420, seed=9)          # 96 < n <= 160: second shared-memory class
+    g3 = synthetic.erdos_renyi(150, 420, seed=9)          # 96 < n <= 160: shared-memory ChFSI (dense: n <= 228)
     views = [[_sub(g1), _sub(g3)], [_sub(g2), _sub(synthetic.path_graph(30))]]
     assert 64 < g1.num_nodes <= 96 < g3.num_nodes <= 160 and 64 < g2.num_nodes
     b, pos, eig = _posenc(views, normalize=0)
@@ -119,6 +127,32 @@ def test_posenc_matches_reference_golden(solver):
             assert np.all(got[:, k:] == 0)
             checked += 1
     assert checked >= 8
+
+
+def test_dense_max_below_96_is_the_default(monkeypatch):
+    """GCCB200_DENSE_MAX below the first dense class acts as 96: the output is bit-identical to the default dispatch's,
+    on ego-nets on both sides of the boundary."""
+    graphs = [synthetic.path_graph(9), synthetic.star_graph(50), synthetic.erdos_renyi(60, 100, seed=4),
+              synthetic.chung_lu(95, 250, seed=2), synthetic.erdos_renyi(150, 420, seed=9),
+              synthetic.chung_lu(156, 420, seed=3)]
+    assert sorted(g.num_nodes > 96 for g in graphs) == [False] * 4 + [True] * 2
+    views = _views(graphs)
+    monkeypatch.delenv("GCCB200_DENSE_MAX", raising=False)
+    _, pos, eig = _posenc(views, normalize=1)
+    monkeypatch.setenv("GCCB200_DENSE_MAX", "0")
+    _, pos0, eig0 = _posenc(views, normalize=1)
+    assert np.array_equal(pos, pos0, equal_nan=True) and np.array_equal(eig, eig0, equal_nan=True)
+
+
+def test_posenc_refuses_a_misaligned_workspace():
+    """The debug area at the start of the workspace holds int64 counters."""
+    L = lib()
+    b = NpBatch.from_subgraphs(_views([synthetic.path_graph(9), synthetic.path_graph(5)]))
+    pos = np.zeros((2, b.node_cap, 32), np.float32)
+    ws = np.zeros(L.gccb_posenc_workspace(b.B, b.node_cap) + 8, np.uint8)
+    assert L.gccb_posenc(C.byref(b.c), 32, 1, ptr(pos), None, C.c_void_p(ws.ctypes.data + 4), ws.nbytes - 4,
+                         None) != 0
+    assert b"aligned" in L.gccb_last_error()
 
 
 def test_huge_egonet_one_block_in_shared_memory():

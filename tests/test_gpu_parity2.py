@@ -25,22 +25,34 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 #   Inside that cluster (spread up to ~1e-3) WHICH members make the top-32 cut is not resolved either, so the
 #   eigenvalue bar for n > 160 is the cluster spread, 1e-3 (2e-5 everywhere else).
 RES_SMALL, RES_HUB, HUB_N, LAM_SMALL, LAM_HUB = 1e-4, 2.5e-3, 160, 2e-5, 1e-3
-# The dense tridiagonal solver (posenc.cu solver (0); GCCB200_DENSE_MAX=228 here, product default 96) is a direct method: eigenvalues to 2e-6,
-# residuals and orthonormality to 2e-5 (measured on the fp32 model: 5e-7 / 4e-6 / 3e-6), hub-like ego-nets included.
-DENSE_N, RES_DENSE, LAM_DENSE = 228, 2e-5, 2e-6
+# The dense tridiagonal solver (posenc.cu solver (0); n <= 96 by default, GCCB200_DENSE_MAX=228 up to 228) is a direct
+# method: eigenvalues to 2e-6, residuals and orthonormality to 2e-5 (measured on the fp32 model: 5e-7 / 4e-6 / 3e-6),
+# hub-like ego-nets included.
+DENSE_N, RES_DENSE, LAM_DENSE = {"default": 96, "dense": 228}, 2e-5, 2e-6
 
 
-@pytest.fixture(params=["dense", "iterative"])
+@pytest.fixture(params=["default", "dense"])
 def solver(request, monkeypatch):
-    """gccb_posenc reads GCCB200_DENSE_MAX on every call: 0 sends every size to the Jacobi / ChFSI classes."""
-    monkeypatch.setenv("GCCB200_DENSE_MAX", "0" if request.param == "iterative" else "228")
+    """gccb_posenc reads GCCB200_DENSE_MAX on every call: unset is the shipped dispatch, 228 sends every ego-net up
+    to 228 vertices to the dense solver."""
+    if request.param == "dense":
+        monkeypatch.setenv("GCCB200_DENSE_MAX", "228")
+    else:
+        monkeypatch.delenv("GCCB200_DENSE_MAX", raising=False)
     return request.param
 
 
 def _bars(n, solver):
-    if solver == "dense" and n <= DENSE_N:
+    if n <= DENSE_N[solver]:
         return RES_DENSE, LAM_DENSE
     return (RES_HUB, LAM_HUB) if n > HUB_N else (RES_SMALL, LAM_SMALL)
+
+
+def _eig_class(n, solver):
+    """The size class posenc.cu sends an n-vertex ego-net to (eig_class)."""
+    if n <= DENSE_N[solver]:
+        return "dense<=%d" % next(c for c in (96, 144, 228) if n <= c)
+    return "chfsi<=%s" % next((c for c in (160, 384, 1536, 3584) if n <= c), "L2")
 
 
 def _spectral(sub, u, lam, res_bar, tol_l):
@@ -69,9 +81,9 @@ def _posenc_raw(buf):
 
 
 def test_eigensolver_every_size_class(solver):
-    """One explicit ego-net per solver class: dense Jacobi (n 40), shared-memory ChFSI (90, 150, 300),
-    cluster ChFSI with 192- and 448-row slabs (520, 1500, 3300) and a 700-vertex star (eigenvalue 0 x 698);
-    with the dense solver on, the first three go through its three classes (n <= 96 / 144 / 228)."""
+    """One explicit ego-net per solver class: the dense solver (n 40, 93), shared-memory ChFSI (152, 309), cluster
+    ChFSI with 192-row slabs (505, 1445, and a 701-vertex star: eigenvalue 0 x 699) and 448-row slabs (2859); with
+    the dense solver up to 228, the 152-vertex ego-net goes through its n <= 228 class instead."""
     from gcc_b200.datasets import synthetic
     from gcc_b200.datasets.graph_dataset import BatchBuffers
     graphs = [synthetic.erdos_renyi(40, 90, seed=1), synthetic.chung_lu(95, 250, seed=2),
@@ -80,8 +92,10 @@ def test_eigensolver_every_size_class(solver):
               synthetic.chung_lu(3500, 9000, exponent=0.9, seed=5), synthetic.star_graph(700)]
     subs = [dict(indptr=g.indptr.astype(np.int32), indices=g.indices.astype(np.int32), n=g.num_nodes) for g in graphs]
     sizes = [s["n"] for s in subs]
-    cls = [0 if n <= 64 else 1 if n <= 96 else 2 if n <= 160 else 3 if n <= 384 else 4 if n <= 1536 else 5 for n in sizes]
-    assert sorted(set(cls)) == [0, 1, 2, 3, 4, 5], (sizes, cls)
+    cls = [_eig_class(n, solver) for n in sizes]
+    want = {"default": ["chfsi<=1536", "chfsi<=160", "chfsi<=3584", "chfsi<=384", "dense<=96"],
+            "dense": ["chfsi<=1536", "chfsi<=3584", "chfsi<=384", "dense<=228", "dense<=96"]}
+    assert sorted(set(cls)) == want[solver], (sizes, cls)
     B = 4
     views = [subs[:4], subs[4:]]
     N = max(sum(s["n"] for s in v) for v in views)
@@ -116,7 +130,7 @@ def test_dense_eigensolver_class_boundaries(monkeypatch):
     subs = [dict(indptr=g.indptr.astype(np.int32), indices=g.indices.astype(np.int32), n=g.num_nodes) for g in graphs]
     z = np.load(os.path.join(ROOT, "tests", "golden", "egonet_cluster15.npz"))
     subs.append(dict(indptr=z["indptr"].astype(np.int32), indices=z["indices"].astype(np.int32), n=len(z["indptr"]) - 1))
-    assert max(s["n"] for s in subs) <= DENSE_N
+    assert max(s["n"] for s in subs) <= DENSE_N["dense"]
     B = len(subs) // 2
     views = [subs[:B], subs[B:]]
     N = max(sum(s["n"] for s in v) for v in views)
