@@ -380,8 +380,11 @@ __device__ __forceinline__ void tile_colstats2(const float (&sv)[4][TileCols<NOU
 
 // dz2 = BN_a backward of g3 (written out); dx1 = dz2 W2; g1 = [bn1(z1) > 0] dx1 (written out);
 // column sums of g1 and g1 * z1hat.
+// At hidden 64 at most 64 registers per thread (63, no spills; 80 unbounded, same instructions otherwise): a CTA
+// then takes 16,384 registers and fits on an SM whose eigensolver CTAs leave a quarter of the register file free
+// (three dense n <= 96 CTAs, or a 512-thread ChFSI CTA and a dense one), where an 80-register CTA has to wait.
 template <int H>
-__global__ void __launch_bounds__(256)
+__global__ void __launch_bounds__(256, H == 64 ? 4 : 0)
 gin_bwd_gemm2_kernel(const int32_t* __restrict__ node_off_v, int B, const float* __restrict__ z1,
                      const float* __restrict__ z2, const float* __restrict__ dh,
                      const double* __restrict__ sums_1, const float* __restrict__ g1w,
@@ -692,6 +695,7 @@ static int run_backward(const BwdArgs& a) {
   float* dS = (float*)(a.ws + a.bl.dS);
   float* dpool = (float*)(a.ws + a.bl.dpool);
   float* part = (float*)(a.ws + a.bl.part);
+  float* part1 = (float*)(a.ws + a.bl.part1);
   const float* P = a.params;
   float* G = a.grads;
   const int DW = a.bl.DW;
@@ -703,19 +707,23 @@ static int run_backward(const BwdArgs& a) {
   // stream (two event forks per layer, after GEMM2 and after GEMM1, one join at the end).  g1/dz2
   // alternate between two buffers so that layer l-1 may overwrite nothing the side stream still reads
   // from layer l; layer l-2 waits for the side work of layer l before reusing its buffers.
+  // dW1 runs on a second side stream with its own split-K partials: behind dW2 and the BatchNorm gradients on
+  // one stream it started late, and the last layer's dW1 held the final join (before the optimiser).  The
+  // second stream follows the first (ev_dw2) before it signals a layer done (ev_side) and before the join.
 #ifndef GCCB_EMU
   // The side stream runs one step above the caller's priority: its kernels are short (one wave of CTAs), and
   // at equal priority they queued behind the next chain kernel's CTAs, so the side stream fell behind and the
   // final join (before the optimiser) waited for the last layers' weight gradients.
   StreamKit* kit = stream_kit((cudaStream_t)a.stream, 2, SidePriority::kAboveCaller);
   cudaStream_t main_s = (cudaStream_t)a.stream;
-  gccb_stream_t side = kit->side[0];
+  gccb_stream_t side = kit->side[0], side1 = kit->side[1];
   cudaEvent_t* ev_main = kit->ev;                          // [0..7]  main -> side, per layer
   cudaEvent_t* ev_side = kit->ev + 8;                      // [8..15] side -> main, per layer
   cudaEvent_t ev_head = kit->ev[16], ev_join = kit->ev[17];
   cudaEvent_t ev_gemm2 = kit->ev[18];                      // main -> side after GEMM2, re-recorded per layer
+  cudaEvent_t ev_dw2 = kit->ev[19];                        // side -> side1 after a layer's side work, likewise
 #else
-  gccb_stream_t side = a.stream;
+  gccb_stream_t side = a.stream, side1 = a.stream;
 #endif
   cudaMemsetAsync(red, 0, (size_t)(d.L - 1) * 3 * 2 * H * sizeof(double), (cudaStream_t)a.stream);
   auto kpb = gin_pool_predict_bwd_kernel<H>;
@@ -801,18 +809,20 @@ static int run_backward(const BwdArgs& a) {
     }
 #ifndef GCCB_EMU
     cudaEventRecord(ev_main[l], main_s);
-    cudaStreamWaitEvent((cudaStream_t)side, ev_main[l], 0);
+    cudaStreamWaitEvent((cudaStream_t)side1, ev_main[l], 0);
 #endif
-    // side stream, once GEMM1 has turned g1 into dz1: dW1 = dz1^T a
+    // second side stream, once GEMM1 has turned g1 into dz1: dW1 = dz1^T a
     {
       dim3 gr1(GCCB_WG_CHUNKS, ((H + 63) / 64) * ((KQ1 + 63) / 64));
-      GCCB_LAUNCH(gin_wgrad_kernel, gr1, 256, 0, side, node_off_v, B, H, KQ1, (const float*)g1, a_l,
-                  (const double*)nullptr, (const float*)nullptr, (const float*)nullptr, d.bn_eps, part);
-      GCCB_LAUNCH(gin_wgrad_reduce_kernel, (H * KQ1 + H + 255) / 256, 256, 0, side, H, KQ1, inf,
-                  (const float*)part, G + a.lay.w1[l], G + a.lay.b1[l]);
+      GCCB_LAUNCH(gin_wgrad_kernel, gr1, 256, 0, side1, node_off_v, B, H, KQ1, (const float*)g1, a_l,
+                  (const double*)nullptr, (const float*)nullptr, (const float*)nullptr, d.bn_eps, part1);
+      GCCB_LAUNCH(gin_wgrad_reduce_kernel, (H * KQ1 + H + 255) / 256, 256, 0, side1, H, KQ1, inf,
+                  (const float*)part1, G + a.lay.w1[l], G + a.lay.b1[l]);
     }
 #ifndef GCCB_EMU
-    cudaEventRecord(ev_side[l], (cudaStream_t)side);
+    cudaEventRecord(ev_dw2, (cudaStream_t)side);
+    cudaStreamWaitEvent((cudaStream_t)side1, ev_dw2, 0);
+    cudaEventRecord(ev_side[l], (cudaStream_t)side1);
 #endif
   }
   // layer-0 input gradient -> degree embedding
@@ -826,7 +836,7 @@ static int run_backward(const BwdArgs& a) {
     GCCB_LAUNCH(k, 64, 256, sm, a.stream, d, node_off_v, B, sub_deg, (const float*)dh, G + a.lay.emb);
   }
 #ifndef GCCB_EMU
-  cudaEventRecord(ev_join, (cudaStream_t)side);
+  cudaEventRecord(ev_join, (cudaStream_t)side1);
   cudaStreamWaitEvent(main_s, ev_join, 0);
 #endif
   return check_launch("gccb_gin_backward");

@@ -73,7 +73,7 @@ inline ActsLayout make_acts_layout(const GinDims& d, int B, int node_cap) {
 #define GCCB_WG_CHUNKS GCCB_NUM_SMS    // row chunks of the weight-gradient split-K (SIMT backward)
 
 struct BwdLayout {            // byte offsets in the backward workspace
-  size_t dh, g1[2], dz2[2], da, red, dS, dpool, part, total;   // g1/dz2 alternate between layers
+  size_t dh, g1[2], dz2[2], da, red, dS, dpool, part, part1, total;   // g1/dz2 alternate between layers
   // tensor-core path: bf16 operand of the input-gradient GEMMs, two transposed bf16 operands of the weight-
   // gradient GEMMs ([W][cap_pad]), per-layer BatchNorm-1 coefficients (sc | sh) and the split-K partials
   size_t dz16, tA, tB, coef1, splitk;
@@ -96,9 +96,10 @@ inline BwdLayout make_bwd_layout(const GinDims& d, int B, int node_cap) {
   b.dS = take((size_t)d.L * B * d.H * 4);
   b.dpool = take((size_t)d.L * B * b.DW * 4);
   b.part = take((size_t)GCCB_WG_CHUNKS * ((size_t)d.H * b.DW + d.H) * 4);
-  b.dz16 = b.tA = b.tB = b.coef1 = b.splitk = 0;
+  b.dz16 = b.tA = b.tB = b.coef1 = b.splitk = b.part1 = 0;
   b.cap_pad = (node_cap + 63) & ~63;
   b.splits = 0;
+  if (!d.tc) b.part1 = take((size_t)GCCB_WG_CHUNKS * ((size_t)d.H * b.DW + d.H) * 4);   // dW1's own stream (SIMT)
 #ifndef GCCB_EMU
   if (d.tc) {
     b.dz16 = take((size_t)node_cap * d.H * 2);

@@ -25,15 +25,37 @@ for k, v in sorted(by.items(), key=lambda kv: -sum(kv[1]))[:34]:
     print("%-62s %5d %9.1f %9.1f %9.3f" % (k, len(v), sum(v) / len(v), max(v), sum(v) / 1e3))
 
 if len(sys.argv) > 2:
-    # sequence view of one step on the busiest GIN stream: start offset, duration, gap to previous
-    main_sid = max(streams, key=lambda k: sum(1 for e in streams[k] if "gin_" in e["name"] or "infonce" in e["name"]))
-    es = streams[main_sid]
-    # one step = between consecutive adam_ema kernels (any stream)
-    adam = sorted(e["ts"] for e in ev if "adam_ema" in e["name"])
-    lo, hi = adam[1], adam[2]
+    def training(e):
+        return any(s in e["name"] for s in ("gin_", "infonce", "update_ema", "moco", "gradnorm"))
+
+    def short(e):
+        return e["name"].split("(")[0].replace("void ", "").replace("gccb::", "")[:50]
+
+    # one step = between consecutive optimiser kernels (any stream)
+    marks = sorted(e["ts"] for e in ev if "update_ema" in e["name"])
+    # idle time on a training stream before each of its kernels (end of the stream's previous kernel -> start),
+    # over every complete step: waits for SM slots show up here, beside waits for other streams' events
+    gaps = collections.defaultdict(list)
+    spans = []
+    for lo, hi in zip(marks, marks[1:]):
+        prev_end = {}
+        inside = [e for e in ev if lo < e["ts"] <= hi and training(e)]
+        spans.append((max(e["ts"] + e["dur"] for e in inside) - min(e["ts"] for e in inside)) if inside else 0.0)
+        for e in inside:
+            sid = e["args"].get("stream")
+            if sid in prev_end:
+                gaps[short(e)].append(e["ts"] - prev_end[sid])
+            prev_end[sid] = max(prev_end.get(sid, 0.0), e["ts"] + e["dur"])
+    nsteps = max(len(marks) - 1, 1)
+    print("%d steps, period %.3f ms, training kernels' span %.3f ms per step; idle gaps before training kernels:" % (
+        len(marks) - 1, (marks[-1] - marks[0]) / 1e3 / nsteps, sum(spans) / 1e3 / nsteps))
+    print("%-52s %5s %9s %9s %13s" % ("kernel", "n", "mean_us", "max_us", "us_per_step"))
+    for k, v in sorted(gaps.items(), key=lambda kv: -sum(kv[1]))[:24]:
+        print("%-52s %5d %9.1f %9.1f %13.1f" % (k, len(v), sum(v) / len(v), max(v), sum(v) / nsteps))
+    print("all gaps: %.1f us per step" % (sum(sum(v) for v in gaps.values()) / nsteps))
+    lo, hi = marks[1], marks[2]
     print("step window %.3f ms; kernels of ALL streams inside it:" % ((hi - lo) / 1e3))
-    inside = [e for e in ev if lo < e["ts"] <= hi and ("gin_" in e["name"] or "infonce" in e["name"] or "adam" in e["name"]
-                                                        or "moco" in e["name"] or "gradnorm" in e["name"])]
+    inside = [e for e in ev if lo < e["ts"] <= hi and training(e)]
     prev_end = {}
     for e in inside:
         sid = e["args"].get("stream")
