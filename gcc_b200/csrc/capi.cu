@@ -3,6 +3,7 @@
 #include <stdio.h>
 
 #include "common.cuh"
+#include <deque>
 #include <mutex>
 
 namespace gccb {
@@ -45,22 +46,23 @@ static cudaStream_t create_stream_like(cudaStream_t like, SidePriority want) {
 }
 
 StreamKit* stream_kit(cudaStream_t caller, int family, SidePriority priority) {
-  static StreamKit kits[16];
-  static int nkits = 0;
+  // one kit per (caller stream, family, device), never shared: the concurrent finetune folds hold three families
+  // on each of ten caller streams, and a kit handed to a second caller (or re-keyed to another device while its
+  // first caller still launches on it) would serialise their side work or put it on another device's streams.
+  // A deque keeps the kits' addresses fixed as it grows.  Kits are never freed: the table is bounded by the distinct
+  // caller-stream handles a process uses, which torch's stream pools keep to a few dozen per device.  A caller that
+  // creates and destroys streams of its own adds a kit (5 streams, 24 events) per new handle, and a recycled handle
+  // reuses the kit keyed by it, which is harmless: a kit holds no state between calls.
+  static std::deque<StreamKit> kits;
   static std::mutex mu;
   std::lock_guard<std::mutex> lock(mu);
   int dev = 0;
   cudaGetDevice(&dev);                                    // streams belong to a device: the legacy stream (0) of two
-  for (int i = 0; i < nkits; ++i)                         // devices must not share side streams
-    if (kits[i].key == caller && kits[i].family == family && kits[i].dev == dev) return &kits[i];
-  StreamKit* k;
-  if (nkits < 16) {
-    k = &kits[nkits++];
-    for (int i = 0; i < 5; ++i) k->side[i] = create_stream_like(caller, priority);
-    for (int i = 0; i < 24; ++i) cudaEventCreateWithFlags(&k->ev[i], cudaEventDisableTiming);
-  } else {
-    k = &kits[15];                                        // more caller streams than kits: share the last one
-  }
+  for (StreamKit& k : kits)                               // devices must not share side streams
+    if (k.key == caller && k.family == family && k.dev == dev) return &k;
+  StreamKit* k = &kits.emplace_back();
+  for (int i = 0; i < 5; ++i) k->side[i] = create_stream_like(caller, priority);
+  for (int i = 0; i < 24; ++i) cudaEventCreateWithFlags(&k->ev[i], cudaEventDisableTiming);
   k->key = caller;
   k->family = family;
   k->dev = dev;

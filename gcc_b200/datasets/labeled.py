@@ -18,6 +18,7 @@ gcc/datasets/data_util.py:35-113,227-236, train.py:516-545).
 The reference downloads its datasets; there is no network here, so `dataset` may also be an in-memory
 object -- (CSRGraph, labels) / (list[CSRGraph], labels) -- or a path.
 """
+import copy
 import ctypes as C
 import os
 from collections import namedtuple
@@ -251,6 +252,20 @@ class _LabeledBase:
     def num_batches(self, n_items, batch_size=None):
         bs = int(batch_size or self.batch_size)
         return (n_items + bs - 1) // bs
+
+    def fold_view(self):
+        """This dataset for one more cross-validation fold on the same device: the read-only device state (graph or
+        union CSR, device labels, whole-graph feature cache) is shared, while the BatchBuffers (and with them the
+        flag word) and the sampler's next_sample counter are the fold's own and start as a freshly built dataset's
+        do, so the fold draws the batches a fresh dataset would give it.  Folds on separate streams may use their
+        views concurrently once the stream that built this dataset has been waited on."""
+        if hasattr(self, "feature_cache"):
+            self.feature_cache()                       # built once, before the views share it
+        view = copy.copy(self)
+        view._bufs = {}
+        if hasattr(self, "next_sample"):
+            view.next_sample = 0
+        return view
 
 
 class NodeClassificationDatasetLabeled(_LabeledBase):

@@ -73,6 +73,7 @@ class FinetuneEngine:
         if hasattr(dataset, "feature_cache"):
             dataset.feature_cache()                    # computed once, before the first step
         self.last_steps = None                         # per-step (loss, f1, rows, nodes, edges) of the last epoch
+        self.out = None                                # where the engine prints (None: sys.stdout)
 
     # -------------------------------------------------------------------------------------------
     def _buffers_scratch(self, buf):
@@ -169,6 +170,17 @@ class FinetuneEngine:
         """One epoch over `order` (the epoch's shuffled train indices) in batches of B, the last one short; the LR of
         batch idx is lr * warmup_linear((epoch * n_batch + idx) / (n_epochs * n_batch), 0.1).  Prints and logs what
         train.train_finetune does; returns (epoch loss, epoch micro-F1)."""
+        steps = self.train_epoch_steps(epoch, order, n_epochs, sw, print_freq, tb_freq)
+        while True:
+            try:
+                next(steps)
+            except StopIteration as done:
+                return done.value
+
+    def train_epoch_steps(self, epoch, order, n_epochs, sw=None, print_freq=10, tb_freq=250):
+        """train_epoch as a generator that yields after issuing each step (and after the reads and prints due at
+        that step), so that one host thread can interleave the steps of several engines on their own streams; its
+        return value is train_epoch's.  Every call to next() must run on the stream of the first."""
         B = self.B
         n = self._load_order(order)
         n_batch = (n + B - 1) // B
@@ -185,6 +197,7 @@ class FinetuneEngine:
             self._step(self.order_dev[a:min(a + B, n)], lr_this_step, log[idx])
             printing, logging = (idx + 1) % print_freq == 0, sw is not None and (idx + 1) % tb_freq == 0
             if not (printing or logging or idx + 1 == n_batch):
+                yield
                 continue
             rows = self._read(log, read_upto, idx + 1, "epoch %d: finetune step" % epoch)
             bt = (time.time() - end) / max(len(rows), 1)
@@ -205,7 +218,8 @@ class FinetuneEngine:
             if printing:
                 print("Train: [{0}][{1}/{2}]\tBT {bt.val:.3f} ({bt.avg:.3f})\tloss {loss.val:.3f} ({loss.avg:.3f})\t"
                       "f1 {f1.val:.3f} ({f1.avg:.3f})\tGS {gs.val:.3f} ({gs.avg:.3f})".format(
-                          epoch, idx + 1, n_batch, bt=batch_time, loss=loss_meter, f1=f1_meter, gs=graph_size))
+                          epoch, idx + 1, n_batch, bt=batch_time, loss=loss_meter, f1=f1_meter, gs=graph_size),
+                      file=self.out)
             if logging:
                 sw.add_scalar("ft_loss", loss_meter.avg, global_step)
                 sw.add_scalar("ft_f1", f1_meter.avg, global_step)
@@ -217,6 +231,7 @@ class FinetuneEngine:
                 f1_meter.reset()
                 graph_size.reset()
                 max_num_nodes = max_num_edges = 0
+            yield
         self.last_steps = steps
         return epoch_loss_meter.avg, epoch_f1_meter.avg
 
@@ -245,7 +260,7 @@ class FinetuneEngine:
         if sw is not None:
             sw.add_scalar("ft_loss/valid", epoch_loss_meter.avg, global_step)
             sw.add_scalar("ft_f1/valid", epoch_f1_meter.avg, global_step)
-        print(f"Epoch {epoch}, loss {epoch_loss_meter.avg:.3f}, f1 {epoch_f1_meter.avg:.3f}")
+        print(f"Epoch {epoch}, loss {epoch_loss_meter.avg:.3f}, f1 {epoch_f1_meter.avg:.3f}", file=self.out)
         return epoch_loss_meter.avg, epoch_f1_meter.avg
 
     def optimizer_state_dict(self):

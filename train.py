@@ -30,12 +30,18 @@ against.
     python train.py --finetune --dataset usa_airport --resume saved/.../current.pth --epochs 30 --fold-idx 0
 """
 import argparse
+import contextlib
+import copy
+import io
 import os
+import sys
+import threading
 import time
 
 import numpy as np
 import torch
 
+from gcc_b200 import _lib
 from gcc_b200.contrastive.memory_moco import MemoryMoCo
 from gcc_b200.datasets import downstream, synthetic
 from gcc_b200.datasets.graph_dataset import (GraphClassificationDataset, LoadBalanceGraphDataset,
@@ -334,15 +340,32 @@ def main_finetune(args, dataset=None):
     """The --finetune branch of the reference's main (train.py:483-545,600-660,716-792): hyper-parameters come
     from the pretraining checkpoint, 10-fold stratified split, BatchNorm running statistics reset, the
     --optimizer for the encoder and Adam for the output layer, validation after the last epoch.  Returns the validation micro-F1."""
-    from sklearn.model_selection import StratifiedKFold
-
-    from gcc_b200.datasets.labeled import (GRAPH_CLASSIFICATION_DSETS, GraphClassificationDatasetLabeled,
-                                           NodeClassificationDatasetLabeled)
     dev = torch.device("cuda", args.gpu[0] if isinstance(args.gpu, (list, tuple)) and args.gpu else (args.gpu or 0))
     torch.cuda.set_device(dev)
     np.random.seed(args.seed)
     torch.manual_seed(args.seed)
     torch.cuda.manual_seed(args.seed)
+    args, checkpoint = _finetune_options(args)
+    if dataset is None:
+        dataset = _labeled_dataset(args, dev)
+    fold = _FinetuneFold(args, checkpoint, dataset, dev)
+    model, engine = fold.model, fold.engine
+    epoch = 0
+    for epoch in range(1, args.epochs + 1):
+        t0 = time.time()
+        loss, _ = engine.train_epoch(epoch, fold.epoch_order(), args.epochs, sw=fold.sw, print_freq=args.print_freq,
+                                     tb_freq=args.tb_freq)
+        print("epoch {}, loss {:.4f}, total time {:.2f}".format(epoch, loss, time.time() - t0))
+        state = {"opt": args, "model": model.state_dict(), "optimizer": engine.optimizer_state_dict(),
+                 "epoch": epoch}
+        _save_finetune_state(args, state, epoch)
+    _, valid_f1 = engine.evaluate(epoch, fold.test_idx, fold.sw)
+    return valid_f1
+
+
+def _finetune_options(args):
+    """main_finetune's options: those of the pretraining checkpoint --resume names win (train.py:491-504), then the
+    run naming.  Returns (args, checkpoint or None)."""
     checkpoint = None
     if args.resume:
         if os.path.isfile(args.resume):
@@ -357,54 +380,234 @@ def main_finetune(args, dataset=None):
             args = pre
         else:
             print("=> no checkpoint found at '{}'".format(args.resume))
-    args = option_update(args)
-    if dataset is None:
-        kw = dict(dataset=args.dataset, rw_hops=args.rw_hops, subgraph_size=args.subgraph_size,
-                  restart_prob=args.restart_prob, positional_embedding_size=args.positional_embedding_size,
-                  device=dev, seed=args.seed, batch_size=args.batch_size)
-        dataset = (GraphClassificationDatasetLabeled(**kw) if args.dataset in GRAPH_CLASSIFICATION_DSETS
-                   else NodeClassificationDatasetLabeled(**kw))
-    labels = dataset.labels.tolist()
-    skf = StratifiedKFold(n_splits=10, shuffle=True, random_state=args.seed)
-    idx_list = list(skf.split(np.zeros(len(labels)), labels))
-    assert 0 <= args.fold_idx < 10, "fold_idx must be from 0 to 9."
-    train_idx, test_idx = idx_list[args.fold_idx]
-    model = _make_encoder(args)
-    if checkpoint is not None:
-        model.load_state_dict(checkpoint["model"])
-    model = model.to(dev)
-    output_layer = torch.nn.Linear(in_features=args.hidden_size, out_features=dataset.num_classes).to(dev)
+    return option_update(args), checkpoint
 
-    def clear_bn(m):                                       # train.py:648-653
-        if m.__class__.__name__.find("BatchNorm") != -1:
-            m.reset_running_stats()
 
-    model.apply(clear_bn)
-    # the --optimizer for the encoder, Adam for the output layer, both after clip_grad_value_(1), every step on the
-    # device (gcc_b200/finetune.py); train_finetune / test_finetune are the same steps with torch ops
-    engine = FinetuneEngine(dataset, model, output_layer, optimizer=args.optimizer, lr=args.learning_rate,
-                            betas=(args.beta1, args.beta2), weight_decay=args.weight_decay, momentum=args.momentum,
-                            lr_decay=args.lr_decay_rate, batch_size=args.batch_size)
-    rng = np.random.RandomState(args.seed)                 # LabeledLoader's shuffle: one permutation per epoch
-    sw = None
-    try:
-        from torch.utils.tensorboard import SummaryWriter
-        sw = SummaryWriter(args.tb_folder)
-    except Exception:
-        sw = None
+def _labeled_dataset(args, dev):
+    from gcc_b200.datasets.labeled import (GRAPH_CLASSIFICATION_DSETS, GraphClassificationDatasetLabeled,
+                                           NodeClassificationDatasetLabeled)
+    kw = dict(dataset=args.dataset, rw_hops=args.rw_hops, subgraph_size=args.subgraph_size,
+              restart_prob=args.restart_prob, positional_embedding_size=args.positional_embedding_size,
+              device=dev, seed=args.seed, batch_size=args.batch_size)
+    return (GraphClassificationDatasetLabeled(**kw) if args.dataset in GRAPH_CLASSIFICATION_DSETS
+            else NodeClassificationDatasetLabeled(**kw))
+
+
+class _FinetuneFold:
+    """One fold of main_finetune (train.py:600-660): the reference's StratifiedKFold(10, shuffle, seed)[fold_idx]
+    split, the encoder (the checkpoint's weights, BatchNorm running statistics reset), the Linear head, the engine
+    (the --optimizer for the encoder, Adam for the output layer, both after clip_grad_value_(1), every step on the
+    device: gcc_b200/finetune.py; train_finetune / test_finetune are the same steps with torch ops), the shuffle's
+    RandomState and the SummaryWriter.  The encoder and head draw their initial weights and dropout key from torch's
+    RNG as it stands at construction."""
+
+    def __init__(self, args, checkpoint, dataset, dev):
+        from sklearn.model_selection import StratifiedKFold
+        labels = dataset.labels.tolist()
+        skf = StratifiedKFold(n_splits=10, shuffle=True, random_state=args.seed)
+        idx_list = list(skf.split(np.zeros(len(labels)), labels))
+        assert 0 <= args.fold_idx < 10, "fold_idx must be from 0 to 9."
+        self.train_idx, self.test_idx = idx_list[args.fold_idx]
+        model = _make_encoder(args)
+        if checkpoint is not None:
+            model.load_state_dict(checkpoint["model"])
+        model = model.to(dev)
+        output_layer = torch.nn.Linear(in_features=args.hidden_size, out_features=dataset.num_classes).to(dev)
+
+        def clear_bn(m):                                   # train.py:648-653
+            if m.__class__.__name__.find("BatchNorm") != -1:
+                m.reset_running_stats()
+
+        model.apply(clear_bn)
+        self.args, self.model, self.output_layer = args, model, output_layer
+        self.engine = FinetuneEngine(dataset, model, output_layer, optimizer=args.optimizer, lr=args.learning_rate,
+                                     betas=(args.beta1, args.beta2), weight_decay=args.weight_decay,
+                                     momentum=args.momentum, lr_decay=args.lr_decay_rate, batch_size=args.batch_size)
+        self.rng = np.random.RandomState(args.seed)       # LabeledLoader's shuffle: one permutation per epoch
+        try:
+            from torch.utils.tensorboard import SummaryWriter
+            self.sw = SummaryWriter(args.tb_folder)
+        except Exception:
+            self.sw = None
+
+    def epoch_order(self):
+        return self.rng.permutation(np.asarray(self.train_idx, dtype=np.int64))
+
+
+def _save_finetune_state(args, state, epoch):
+    torch.save(state, os.path.join(args.model_folder, "current.pth"))
+    if epoch % args.save_freq == 0:
+        torch.save(state, os.path.join(args.model_folder, "ckpt_epoch_{epoch}.pth".format(epoch=epoch)))
+
+
+def fold_gpus(gpus, n_folds=10):
+    """The reference's fold placement (train.py:800-813): fold i runs on gpus[i % len(gpus)] (GPU 0 without --gpu)."""
+    gpus = list(gpus) if gpus else [0]
+    return [gpus[i % len(gpus)] for i in range(n_folds)]
+
+
+class _CheckpointsInFoldOrder:
+    """The folds' per-epoch checkpoints, written to disk in fold order once every fold has reached the epoch, so the
+    files left behind are the serial loop's: every fold writes the same names, and fold 9's come last."""
+
+    def __init__(self, n_folds):
+        self.n_folds, self.pending, self.lock = n_folds, {}, threading.Lock()
+
+    def put(self, fold_idx, epoch, args, state):
+        with self.lock:
+            ready = self.pending.setdefault(epoch, {})
+            ready[fold_idx] = (args, state)
+            if len(ready) == self.n_folds:
+                for f in sorted(ready):
+                    _save_finetune_state(*ready[f], epoch)
+                del self.pending[epoch]
+
+
+class _CvFold:
+    """A fold of the concurrent --cv driver: its place, stream, printed lines and result, and its _FinetuneFold."""
+
+    def __init__(self, idx, gpu):
+        self.idx, self.dev = idx, torch.device("cuda", gpu)
+        self.stream = torch.cuda.Stream(device=self.dev)
+        self.out = io.StringIO()
+        self.run = self.steps = self.loss = self.seconds = self.f1 = self.error = None
+
+
+def _cv_epoch(folds, epoch, epochs):
+    """One training epoch of the folds on one GPU: their steps issued round-robin, one step of each fold in turn,
+    each fold on its own stream, so their launches overlap on the device.  The host reads a fold's step log only where
+    main_finetune reads it (--print-freq, --tb-freq, the end of the epoch).  Sets each fold's .loss and .seconds, or
+    its .error: a GccbError ends that fold's epoch, the others go on."""
+    t0 = time.time()
+    live = []
+    for f in folds:
+        a = f.run.args
+        f.steps = f.run.engine.train_epoch_steps(epoch, f.run.epoch_order(), epochs, sw=f.run.sw,
+                                                 print_freq=a.print_freq, tb_freq=a.tb_freq)
+        live.append(f)
+    while live:
+        for f in list(live):
+            with torch.cuda.stream(f.stream):
+                try:
+                    next(f.steps)
+                    continue
+                except StopIteration as done:
+                    f.loss, f.seconds = done.value[0], time.time() - t0
+                except _lib.GccbError as e:
+                    f.error = _lib.GccbError("fold %d: %s" % (f.idx, e))
+            live.remove(f)
+
+
+def _cv_device_loop(folds, epochs, checkpoints, stop):
+    """Train the folds placed on one GPU epoch by epoch (_cv_epoch), hand each epoch's checkpoints to `checkpoints`,
+    then run each fold's validation pass.  Stops after the epoch in which a fold failed, or once `stop` is set."""
+    torch.cuda.set_device(folds[0].dev)
     epoch = 0
-    for epoch in range(1, args.epochs + 1):
-        t0 = time.time()
-        loss, _ = engine.train_epoch(epoch, rng.permutation(np.asarray(train_idx, dtype=np.int64)), args.epochs,
-                                     sw=sw, print_freq=args.print_freq, tb_freq=args.tb_freq)
-        print("epoch {}, loss {:.4f}, total time {:.2f}".format(epoch, loss, time.time() - t0))
-        state = {"opt": args, "model": model.state_dict(), "optimizer": engine.optimizer_state_dict(),
-                 "epoch": epoch}
-        torch.save(state, os.path.join(args.model_folder, "current.pth"))
-        if epoch % args.save_freq == 0:
-            torch.save(state, os.path.join(args.model_folder, "ckpt_epoch_{epoch}.pth".format(epoch=epoch)))
-    _, valid_f1 = engine.evaluate(epoch, test_idx, sw)
-    return valid_f1
+    for epoch in range(1, epochs + 1):
+        if stop.is_set():
+            return
+        _cv_epoch(folds, epoch, epochs)
+        if any(f.error for f in folds):
+            stop.set()
+            return
+        for f in folds:
+            print("epoch {}, loss {:.4f}, total time {:.2f}".format(epoch, f.loss, f.seconds), file=f.out)
+            with torch.cuda.stream(f.stream):
+                # copies of the state on the device, as the serial loop saves it (views of one flat buffer stay so)
+                state = {"opt": f.run.args, "model": copy.deepcopy(f.run.model.state_dict()),
+                         "optimizer": f.run.engine.optimizer_state_dict(), "epoch": epoch}
+            f.stream.synchronize()                         # the writer reads them on another stream
+            checkpoints.put(f.idx, epoch, f.run.args, state)
+    for f in folds:
+        with torch.cuda.stream(f.stream):
+            try:
+                _, f.f1 = f.run.engine.evaluate(epoch, f.run.test_idx, f.run.sw)
+            except _lib.GccbError as e:
+                f.error = _lib.GccbError("fold %d: %s" % (f.idx, e))
+
+
+def main_finetune_cv(args, datasets=None, n_folds=10):
+    """--finetune --cv: main_finetune's ten folds run concurrently and return their validation micro-F1 in fold order.
+    Fold i runs on GPU gpus[i % len(gpus)] (fold_gpus), each with its own stream, engine, encoder, head, optimiser
+    state, shuffle RandomState and SummaryWriter, built as main_finetune builds them for --fold-idx i: torch is seeded
+    with the command line's --seed before each fold's encoder, as main_finetune seeds it before a --resume checkpoint's
+    options replace the command line's.  Each GPU builds the labeled dataset once (`datasets`: an optional
+    {gpu: dataset} instead); the folds there share its read-only device state through fold_view() and own their
+    batch buffers and sampler counter, so every fold runs the batches and arithmetic of its solo run.  One host thread
+    per GPU issues its folds' steps round-robin.  Each fold's printed lines are held and written as one block per fold,
+    in fold order, when the run ends, however it ends; the checkpoints are written in fold order
+    (_CheckpointsInFoldOrder).  A fold's GccbError, in training or validation, names the fold; the first in fold order
+    is raised after the blocks of the folds before it and its own."""
+    seed = args.seed                                       # main_finetune seeds before _finetune_options
+    placement = fold_gpus(args.gpu, n_folds)
+    folds = [_CvFold(i, g) for i, g in enumerate(placement)]
+    try:
+        shared = {}
+        for f in folds:                                    # on the main thread: torch's RNG is process-wide
+            a = copy.deepcopy(args)
+            a.fold_idx = f.idx
+            with torch.cuda.device(f.dev), contextlib.redirect_stdout(f.out):
+                a, checkpoint = _finetune_options(a)
+                if f.dev.index not in shared:
+                    ds = (datasets or {}).get(f.dev.index)
+                    shared[f.dev.index] = ds if ds is not None else _labeled_dataset(a, f.dev)
+                view = shared[f.dev.index].fold_view()
+                f.stream.wait_stream(torch.cuda.current_stream(f.dev))  # the shared state is built on this stream
+                np.random.seed(seed)
+                torch.manual_seed(seed)
+                torch.cuda.manual_seed(seed)
+                with torch.cuda.stream(f.stream):
+                    f.run = _FinetuneFold(a, checkpoint, view, f.dev)
+            f.run.engine.out = f.out
+        checkpoints, stop = _CheckpointsInFoldOrder(n_folds), threading.Event()
+        by_gpu = {}
+        for f in folds:
+            by_gpu.setdefault(f.dev.index, []).append(f)
+        groups = list(by_gpu.values())
+        crashed = []
+
+        def work(group):
+            try:
+                _cv_device_loop(group, args.epochs, checkpoints, stop)
+            except BaseException as e:                     # reraised on the main thread
+                stop.set()
+                crashed.append(e)
+
+        if len(groups) == 1:
+            _cv_device_loop(groups[0], args.epochs, checkpoints, stop)
+        else:
+            threads = [threading.Thread(target=work, args=(g,)) for g in groups]
+            for t in threads:
+                t.start()
+            for t in threads:
+                t.join()
+            if crashed:
+                raise crashed[0]
+    finally:
+        for f in folds:
+            sys.stdout.write(f.out.getvalue())
+            if f.error is not None:
+                break
+    for f in folds:
+        if f.error is not None:
+            raise f.error
+    return [f.f1 for f in folds]
+
+
+def finetune_cv_serial(args, make_dataset=None):
+    """--finetune --cv one fold after another, each fold building a dataset of its own (the loop of
+    train.py:801-816): what main_finetune_cv is checked and timed against.  make_dataset(device), if given, builds the
+    fold's dataset in place of --dataset's."""
+    f1 = []
+    for fold_idx in range(10):
+        a = copy.deepcopy(args)
+        a.fold_idx = fold_idx
+        if make_dataset is None:
+            f1.append(main(a))
+        else:
+            gpu = a.gpu[0] if isinstance(a.gpu, (list, tuple)) and a.gpu else (a.gpu or 0)
+            f1.append(main_finetune(a, dataset=make_dataset(torch.device("cuda", gpu))))
+    return f1
 
 
 def main(args):
@@ -477,12 +680,7 @@ def main(args):
 if __name__ == "__main__":
     _args = parse_option()
     if _args.cv and _args.finetune:                         # train.py:801-816
-        import copy
-        f1 = []
-        for fold_idx in range(10):
-            a = copy.deepcopy(_args)
-            a.fold_idx = fold_idx
-            f1.append(main(a))
+        f1 = main_finetune_cv(_args)
         print(f1)
         print(f"Mean = {np.mean(f1)}; Std = {np.std(f1)}")
     else:
