@@ -117,8 +117,11 @@ def _check(Lb, cfg, b, views, pos, seed=0):
             assert np.allclose(got, want, rtol=1e-3, atol=1e-4 * scale), (view, k_, np.abs(got - want).max(), scale)
 
 
-@pytest.mark.parametrize("L,H,nh,T,K", [(2, 32, 4, 2, 2), (3, 64, 1, 2, 1), (2, 128, 8, 1, 3), (2, 64, 4, 6, 3)])
+@pytest.mark.parametrize("L,H,nh,T,K", [(2, 32, 4, 2, 2), (3, 64, 1, 2, 1), (2, 128, 8, 1, 3), (2, 64, 4, 6, 3),
+                                        (1, 256, 8, 2, 1), (1, 32, 2, 1, 1), (2, 256, 1, 2, 2), (1, 64, 4, 3, 8)])
 def test_sampled_batch_vs_oracle(L, H, nh, T, K):
+    """Every head width F = H / nh from 4 (8 heads at 32) to 256 (head_sum's F > 32 branch), one layer (the top
+    layer is layer 0: dX0 comes straight from the Set2Set gradient), and GAT_MAXK = 8 LSTM layers."""
     b, views, pos = _batch(4, 12)
     cfg = glayout.make_gat_cfg(num_layers=L, hidden=H, num_heads=nh, set2set_iter=T, set2set_layers=K)
     _check(lib(), cfg, b, views, pos, seed=L * 7 + H)
