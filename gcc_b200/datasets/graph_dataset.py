@@ -104,6 +104,14 @@ class DeviceGraph:
         self.nbytes = self.indptr.numel() * 8 + self.indices.numel() * 4
 
 
+def walk_capacity(B, max_budget, node_cap=None, edge_cap=None, clip=None):
+    """(node_cap, edge_cap) for B walks of budget <= max_budget, unless given: B ego-nets of max_budget + HOPCAP
+    vertices (on average at most `clip`, if given) plus one more, and 16 edge slots per vertex."""
+    per = max_budget + HOPCAP
+    node_cap = int(node_cap or B * (per if clip is None else min(per, clip)) + per)
+    return node_cap, int(edge_cap or node_cap * 16)
+
+
 class BatchBuffers:
     """Caller-owned device memory behind one gccb_batch_t (both views of B pairs).  max_budget sizes the
     sampler's workspace; None for buffers that only whole-graph batches fill (gccb_gather_graphs needs none)."""
@@ -161,6 +169,21 @@ class BatchBuffers:
             self._narrowed[b] = s
         return self._narrowed[b]
 
+    def posenc(self):
+        """Positional features of both views of the batch these buffers hold (data_util.py:242-281), on the
+        current stream."""
+        _lib.check(_lib.get().gccb_posenc(C.byref(self.c), self.pos_dim, 1, _lib.dptr(self.pos),
+                                          _lib.dptr(self.eigvals), _lib.dptr(self.ws_posenc),
+                                          self.ws_posenc.numel(), _lib.stream_ptr()), "gccb_posenc")
+
+    def mark_absent(self, view):
+        """Mark view `view` absent for the eigensolver, which then solves the other view alone: zero offsets and
+        counters, node_off[view, B] = -1 (posenc.cu classify kernel)."""
+        self.node_off[view].zero_()
+        self.edge_off[view].zero_()
+        self.node_off[view, self.B] = -1
+        self.counters[view * self.B:(view + 1) * self.B].zero_()
+
     def eig_debug(self):
         """(iterations, worst residual) per ego-net of the last gccb_posenc on these buffers, read
         from the debug area at the start of its workspace (posenc.cu: phase[2B][8] int64 | iters[2B] int32 |
@@ -207,12 +230,19 @@ def step_cdf(step_dist):
     return np.ascontiguousarray(cdf / cdf[-1])
 
 
-def sample_views(ds, buf, st):
-    """Both views of buf's B pairs from buf.seeds / buf.sample_ids, as `ds` asks: its step_cdf (None: the k view
-    shares the seed; else gccb_pair_seeds draws buf.seeds_k on the device) and its aug ("rwr": gccb_sample_batch, or
-    gccb_sample_batch_pairs for separate seeds; "ns": gccb_ns_batch).  No host sync."""
-    lib = _lib.get()
-    g = ds.graph
+def sample_pairs(ds, buf, first_sample, seeds=None):
+    """Both views of buf's B pairs with sample ids first_sample.., walked on ds.graph with no host sync.  Seeds: drawn
+    (gccb_draw_seeds), or `seeds` (device int64 [B], or buf.seeds already written).  Views: by ds.step_cdf (None: the
+    k view shares the seed; else gccb_pair_seeds draws buf.seeds_k) and ds.aug ("rwr": gccb_sample_batch, or
+    gccb_sample_batch_pairs for separate seeds; "ns": gccb_ns_batch).  Returns buf."""
+    lib, st, g = _lib.get(), _lib.stream_ptr(), ds.graph
+    if seeds is None:
+        _lib.check(lib.gccb_draw_seeds(_lib.dptr(g.cdf), g.num_nodes, g.key, int(first_sample), buf.B,
+                                       _lib.dptr(buf.seeds), _lib.dptr(buf.sample_ids), st), "gccb_draw_seeds")
+    else:
+        if seeds is not buf.seeds:
+            buf.seeds.copy_(seeds, non_blocking=True)
+        torch.arange(first_sample, first_sample + buf.B, device=buf.seeds.device, out=buf.sample_ids)
     cdf, aug = getattr(ds, "step_cdf", None), getattr(ds, "aug", "rwr")   # the labeled datasets: the defaults
     seeds_k = buf.seeds
     if cdf is not None:
@@ -231,6 +261,7 @@ def sample_views(ds, buf, st):
         _lib.check(lib.gccb_sample_batch_pairs(C.byref(g.c), _lib.dptr(buf.seeds), _lib.dptr(seeds_k),
                                                _lib.dptr(buf.sample_ids), C.byref(buf.c), *ws),
                    "gccb_sample_batch_pairs")
+    return buf
 
 
 class LoadBalanceGraphDataset(torch.utils.data.IterableDataset):
@@ -285,8 +316,7 @@ class LoadBalanceGraphDataset(torch.utils.data.IterableDataset):
         self.graph = DeviceGraph(graph, rw_hops, restart_prob, self.seed, self.device, budget_cap=budget_cap)
         B = self.batch_size
         mb = self.graph.max_budget
-        self.node_cap = int(node_cap or (B * min(mb + HOPCAP, 320) + mb + HOPCAP))
-        self.edge_cap = int(edge_cap or self.node_cap * 16)
+        self.node_cap, self.edge_cap = walk_capacity(B, mb, node_cap, edge_cap, clip=320)
         if aug == "ns":
             # the ns workspace holds ego-nets of up to ego_cap vertices: sizing the buffers' sampler workspace as for
             # that walk budget gives every copy of them (PretrainEngine's run-ahead ring) room for it
@@ -307,31 +337,18 @@ class LoadBalanceGraphDataset(torch.utils.data.IterableDataset):
     def sample_batch(self, first_sample=None, seeds=None, buffers=None, posenc=True):
         """Draw (or take) B seeds, walk, induce, batch and compute positional features for both
         views.  Returns the BatchBuffers (device).  `seeds`: optional int64 tensor [B]."""
-        lib = _lib.get()
         buf = buffers or self.buffers
-        B = buf.B
-        st = _lib.stream_ptr()
         if first_sample is None:
             first_sample = self.next_sample
-            self.next_sample += B
-        if seeds is None:
-            _lib.check(lib.gccb_draw_seeds(_lib.dptr(self.graph.cdf), self.graph.num_nodes,
-                                           self.graph.key, int(first_sample), B, _lib.dptr(buf.seeds),
-                                           _lib.dptr(buf.sample_ids), st), "gccb_draw_seeds")
-        else:
-            buf.seeds.copy_(seeds, non_blocking=True)
-            buf.sample_ids.copy_(torch.arange(first_sample, first_sample + B, device=self.device))
-        sample_views(self, buf, st)
+            self.next_sample += buf.B
+        sample_pairs(self, buf, first_sample, seeds)
         if posenc:
-            self.posenc(buf)
+            buf.posenc()
         return buf
 
     def posenc(self, buffers=None):
-        """Positional features of both views of a sampled batch (data_util.py:242-281)."""
-        buf = buffers or self.buffers
-        _lib.check(_lib.get().gccb_posenc(C.byref(buf.c), buf.pos_dim, 1, _lib.dptr(buf.pos),
-                                          _lib.dptr(buf.eigvals), _lib.dptr(buf.ws_posenc),
-                                          buf.ws_posenc.numel(), _lib.stream_ptr()), "gccb_posenc")
+        """Positional features of both views of a sampled batch (BatchBuffers.posenc)."""
+        (buffers or self.buffers).posenc()
 
     def __iter__(self):
         """Yields batched (graph_q, graph_k) -- what DataLoader(collate_fn=batcher()) yields in the
@@ -349,6 +366,13 @@ class _EpochOrder:
     trains these datasets on one GPU only, so the engine refuses world_size > 1 for them."""
 
     epoch_ordered = True
+
+    def __len__(self):
+        return self.length
+
+    def posenc(self, buffers=None):
+        """Positional features of both views of a batch (BatchBuffers.posenc)."""
+        (buffers or self.buffers).posenc()
 
     def steps_per_epoch(self):
         return -(-self.total // self.batch_size)
@@ -389,21 +413,17 @@ class NodeClassificationDataset(_EpochOrder):
         self.length = self.total = self.graph.num_nodes
         self.batch_size = B = int(min(batch_size, self.length))
         mb = self.graph.max_budget
-        self.node_cap = int(node_cap or (B * min(mb + HOPCAP, 320) + mb + HOPCAP))
-        self.edge_cap = int(edge_cap or self.node_cap * 16)
+        self.node_cap, self.edge_cap = walk_capacity(B, mb, node_cap, edge_cap, clip=320)
         self.buffers = BatchBuffers(B, self.node_cap, self.edge_cap, positional_embedding_size, mb, self.device)
-        self._sampler = LoadBalanceGraphDataset.sample_batch
         self.next_batch = 0
-
-    def __len__(self):
-        return self.length
 
     def __iter__(self):
         B = self.batch_size
         for start in range(0, self.length, B):
             count = min(B, self.length - start)
             seeds = torch.arange(start, start + B, device=self.device).clamp_(max=self.length - 1)
-            buf = self._sampler(self, first_sample=start, seeds=seeds)
+            buf = sample_pairs(self, self.buffers, start, seeds)
+            buf.posenc()
             buf.check_flags()
             yield BatchedSubgraphs(buf, 0), BatchedSubgraphs(buf, 1), count
 
@@ -416,14 +436,10 @@ class NodeClassificationDataset(_EpochOrder):
         epoch, a, b = self._locate(first_sample)
         buf = (buffers or self.buffers).narrow(b)
         torch.arange(a, a + b, device=self.device, out=buf.seeds)
-        base = epoch * self.total
-        torch.arange(base + a, base + a + b, device=self.device, out=buf.sample_ids)
-        sample_views(self, buf, _lib.stream_ptr())
+        sample_pairs(self, buf, epoch * self.total + a, buf.seeds)
         if posenc:
-            self.posenc(buf)
+            buf.posenc()
         return buf
-
-    posenc = LoadBalanceGraphDataset.posenc
 
 
 def seed_first_union(graphs):
@@ -438,6 +454,64 @@ def seed_first_union(graphs):
     indptr = np.concatenate([ip[:-1] + e for (ip, _), e in zip(items, edge_off)] + [edge_off[-1:]])
     indices = np.concatenate([np.asarray(ix, dtype=np.int64) + a for (_, ix), a in zip(items, node_off)])
     return seeds, items, indptr.astype(np.int64), indices, node_off, edge_off
+
+
+class DeviceGraphSet:
+    """Whole graphs relabelled seed first (seed_first_union; seeds, items, node offsets, sizes kept on the host), their
+    union CSR on the device as a gccb_graph_set_t, and the positional-feature cache (rows per vertex, eigenvalues per
+    graph).  Datasets and their fold views share one by reference."""
+
+    def __init__(self, graphs, device):
+        self.device = torch.device(device)
+        self.seeds, self.items, indptr, indices, self.node_off_host, edge_off = seed_first_union(graphs)
+        self.sizes, self.nnz = np.diff(self.node_off_host), np.diff(edge_off)
+        to = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a)).to(device=self.device, dtype=dt)
+        self.indptr, self.indices = to(indptr, torch.int64), to(indices, torch.int32)
+        self.node_off, self.edge_off = to(self.node_off_host, torch.int64), to(edge_off, torch.int64)
+        self.c = _capi.GraphSet(self.indptr.data_ptr(), self.indices.data_ptr(), self.node_off.data_ptr(),
+                                self.edge_off.data_ptr(), len(graphs))
+        self.features = self.eigvals = None
+
+    def buffers(self, B, pos_dim):
+        """BatchBuffers that hold any B graphs of the set: the capacity of the B largest, plus 8, and no sampler
+        workspace (gccb_gather_graphs needs none)."""
+        top = lambda counts: int(np.sort(counts)[::-1][:B].sum()) + 8
+        return BatchBuffers(B, top(self.sizes), top(self.nnz), pos_dim, None, self.device)
+
+    def gather(self, ids, buf):
+        """Both views of buf's batch are the graphs `ids` (device int64 [buf.B]): gccb_gather_graphs, no host sync."""
+        _lib.check(_lib.get().gccb_gather_graphs(C.byref(self.c), _lib.dptr(ids), C.byref(buf.c), _lib.stream_ptr()),
+                   "gccb_gather_graphs")
+
+    def feature_cache(self, pos_dim, B):
+        """Positional features of every vertex of the union [vertices][pos_dim] (and self.eigvals [graphs][pos_dim]),
+        computed on first use, in batches of B consecutive ids, whose rows are the union's rows in order.  The
+        eigensolver is deterministic, so these are what gccb_posenc computes for a graph in any batch."""
+        if self.features is None:
+            no, n = self.node_off_host, len(self.items)
+            cache = torch.empty(int(no[-1]), pos_dim, dtype=torch.float32, device=self.device)
+            eigvals = torch.empty(n, pos_dim, dtype=torch.float32, device=self.device)
+            full = self.buffers(B, pos_dim)
+            ids = torch.arange(n, dtype=torch.int64, device=self.device)
+            for a in range(0, n, B):
+                b = min(B, n - a)
+                buf = full.narrow(b)
+                self.gather(ids[a:a + b], buf)
+                buf.mark_absent(1)
+                buf.posenc()
+                cache[no[a]:no[a + b]].copy_(buf.pos[0, :no[a + b] - no[a]])
+                eigvals[a:a + b].copy_(buf.eigvals[:b])
+            full.check_flags()
+            self.features, self.eigvals = cache, eigvals
+        return self.features
+
+    def gather_features(self, ids, buf):
+        """View 0's positional rows (gccb_gather_features) and eigenvalues of the graphs `ids` (device int64 [buf.B])
+        from the feature cache, which feature_cache() has built.  No host sync."""
+        _lib.check(_lib.get().gccb_gather_features(C.byref(self.c), _lib.dptr(ids), C.byref(buf.c), 0,
+                                                   _lib.dptr(self.features), buf.pos_dim, _lib.dptr(buf.pos),
+                                                   _lib.stream_ptr()), "gccb_gather_features")
+        torch.index_select(self.eigvals, 0, ids, out=buf.eigvals[:buf.B])
 
 
 class GraphClassificationDataset(_EpochOrder):
@@ -467,24 +541,14 @@ class GraphClassificationDataset(_EpochOrder):
         else:
             graphs = list(dataset)
         self.length = self.total = len(graphs)
-        self.seeds, self.items, indptr, indices, node_off, edge_off = seed_first_union(graphs)
-        sizes, nnz = np.diff(node_off), np.diff(edge_off)
         self.device = torch.device(device)
         _lib.require_device()
-        to = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a)).to(device=self.device, dtype=dt)
-        self.indptr, self.indices = to(indptr, torch.int64), to(indices, torch.int32)
-        self.node_off, self.edge_off = to(node_off, torch.int64), to(edge_off, torch.int64)
-        self.c = _capi.GraphSet(self.indptr.data_ptr(), self.indices.data_ptr(), self.node_off.data_ptr(),
-                                self.edge_off.data_ptr(), self.total)
+        self.graph_set = DeviceGraphSet(graphs, self.device)
+        self.seeds, self.items = self.graph_set.seeds, self.graph_set.items      # each item's seed and graph
         self.batch_size = B = int(min(batch_size, self.total))
-        # capacity of the B largest graphs (labeled.GraphClassificationDatasetLabeled._new_buffers)
-        self.node_cap = int(np.sort(sizes)[::-1][:B].sum()) + 8
-        self.edge_cap = int(np.sort(nnz)[::-1][:B].sum()) + 8
-        self.buffers = BatchBuffers(B, self.node_cap, self.edge_cap, positional_embedding_size, None, self.device)
+        self.buffers = self.graph_set.buffers(B, positional_embedding_size)
+        self.node_cap, self.edge_cap = self.buffers.node_cap, self.buffers.edge_cap
         self.next_batch = 0
-
-    def __len__(self):
-        return self.length
 
     def sample_batch(self, first_sample=None, seeds=None, buffers=None, posenc=True):
         """Batch number first_sample // B of the epoch order: graphs a .. a+b-1 in both views, on the device with
@@ -494,10 +558,7 @@ class GraphClassificationDataset(_EpochOrder):
         _, a, b = self._locate(first_sample)
         buf = (buffers or self.buffers).narrow(b)
         torch.arange(a, a + b, device=self.device, out=buf.seeds)
-        _lib.check(_lib.get().gccb_gather_graphs(C.byref(self.c), _lib.dptr(buf.seeds), C.byref(buf.c),
-                                                 _lib.stream_ptr()), "gccb_gather_graphs")
+        self.graph_set.gather(buf.seeds, buf)
         if posenc:
-            self.posenc(buf)
+            buf.posenc()
         return buf
-
-    posenc = LoadBalanceGraphDataset.posenc

@@ -19,17 +19,16 @@ The reference downloads its datasets; there is no network here, so `dataset` may
 object -- (CSRGraph, labels) / (list[CSRGraph], labels) -- or a path.
 """
 import copy
-import ctypes as C
 import os
 from collections import namedtuple
 
 import numpy as np
 import torch
 
-from .. import _capi, _lib
+from .. import _lib
 from . import synthetic
 from .data_util import BatchedSubgraphs
-from .graph_dataset import HOPCAP, BatchBuffers, DeviceGraph, LoadBalanceGraphDataset, seed_first_union
+from .graph_dataset import BatchBuffers, DeviceGraph, DeviceGraphSet, sample_pairs, walk_capacity
 
 Data = namedtuple("Data", ["x", "edge_index", "y"])          # data_util.py:44
 
@@ -100,12 +99,7 @@ def graph_from_edge_index(edge_index, num_nodes=None):
     are dropped like x2dgl.py does for the pretraining corpus (a multi-edge only changes walk probabilities)."""
     src, dst = (np.asarray(a, dtype=np.int64) for a in edge_index)
     n = int(max(src.max(), dst.max())) + 1 if num_nodes is None else int(num_nodes)
-    keep = src != dst
-    key = np.unique(np.concatenate([src[keep] * n + dst[keep], dst[keep] * n + src[keep]]))
-    s, d = key // n, key % n
-    indptr = np.zeros(n + 1, dtype=np.int64)
-    np.cumsum(np.bincount(s, minlength=n), out=indptr[1:])
-    return synthetic.CSRGraph(indptr, d.astype(np.int32), n, "edge_index")
+    return _simple_csr(src, dst, n, "edge_index")
 
 
 def read_tu_dataset(root, name, multigraph=False):
@@ -180,7 +174,7 @@ def seed_first(indptr, indices, seed):
 def fill_whole_graphs(buf, graphs, view=0):
     """Write whole (already relabelled) graphs into view `view` of a BatchBuffers as one batch; the other view
     is marked absent for the eigensolver (node_off[.., B] = -1, posenc.cu classify kernel).  Host-side
-    assembly: the finetune datasets hold a few thousand small graphs."""
+    assembly, the reference the tests hold gccb_gather_graphs (DeviceGraphSet.gather) to."""
     B = buf.B
     assert len(graphs) == B
     sizes = np.array([len(g[0]) - 1 for g in graphs], dtype=np.int64)
@@ -214,16 +208,8 @@ def fill_whole_graphs(buf, graphs, view=0):
     cnt = np.zeros((B, 4), dtype=np.int64)
     cnt[:, 0], cnt[:, 1] = sizes, nnz
     put(buf.counters[view * B:(view + 1) * B], cnt)
-    other = 1 - view
-    buf.node_off[other].zero_()
-    buf.edge_off[other].zero_()
-    buf.node_off[other, B] = -1
-    buf.counters[other * B:(other + 1) * B].zero_()
+    BatchBuffers.mark_absent(buf, 1 - view)        # buf: BatchBuffers, or any object with its arrays
     return buf
-
-
-def _posenc(buf):
-    LoadBalanceGraphDataset.posenc(None, buf)
 
 
 class _LabeledBase:
@@ -249,18 +235,24 @@ class _LabeledBase:
             chunk = idx[a:a + bs]
             yield self._make_batch(chunk), torch.from_numpy(self.labels[chunk]).to(self.device)
 
+    def _make_batch(self, chunk):
+        """device_batch of the host item ids `chunk`, then a host sync that raises on a device flag."""
+        buf = self.device_batch(torch.from_numpy(np.ascontiguousarray(chunk)).to(self.device))
+        buf.check_flags()
+        return BatchedSubgraphs(buf, 0)
+
     def num_batches(self, n_items, batch_size=None):
         bs = int(batch_size or self.batch_size)
         return (n_items + bs - 1) // bs
 
     def fold_view(self):
         """This dataset for one more cross-validation fold on the same device: the read-only device state (graph or
-        union CSR, device labels, whole-graph feature cache) is shared, while the BatchBuffers (and with them the
+        graph set with its feature cache, device labels) is shared, while the BatchBuffers (and with them the
         flag word) and the sampler's next_sample counter are the fold's own and start as a freshly built dataset's
         do, so the fold draws the batches a fresh dataset would give it.  Folds on separate streams may use their
         views concurrently once the stream that built this dataset has been waited on."""
         if hasattr(self, "feature_cache"):
-            self.feature_cache()                       # built once, before the views share it
+            self.feature_cache()                       # built now, on the stream the folds' streams wait on
         view = copy.copy(self)
         view._bufs = {}
         if hasattr(self, "next_sample"):
@@ -316,31 +308,17 @@ class NodeClassificationDatasetLabeled(_LabeledBase):
 
     def _new_buffers(self, B):
         mb = self.graph.max_budget
-        node_cap = int(self._caps[0] or (B * (mb + HOPCAP) + mb + HOPCAP))
-        edge_cap = int(self._caps[1] or node_cap * 16)
-        return BatchBuffers(B, node_cap, edge_cap, self.positional_embedding_size, mb, self.device)
-
-    def _make_batch(self, chunk):
-        buf = self._buffers(len(chunk))
-        seeds = torch.from_numpy(np.ascontiguousarray(chunk)).to(self.device)
-        first = self.next_sample                       # fresh walk randomness for every item drawn, like the reference
-        self.next_sample += len(chunk)
-        LoadBalanceGraphDataset.sample_batch(self, first_sample=first, seeds=seeds, buffers=buf)
-        buf.check_flags()
-        return BatchedSubgraphs(buf, 0)
+        return BatchBuffers(B, *walk_capacity(B, mb, *self._caps), self.positional_embedding_size, mb, self.device)
 
     def device_batch(self, ids):
-        """_make_batch for the items `ids` (device int64 [b]) with no host sync: the same buffers, walks and
-        features.  A batch over its capacity is published empty with the buffers' flag raised; the caller reads
-        the flag."""
-        b = ids.numel()
-        buf = self._buffers(b)
-        first = self.next_sample
-        self.next_sample += b
-        LoadBalanceGraphDataset.sample_batch(self, first_sample=first, seeds=ids, buffers=buf)
+        """Ego-nets of the items `ids` (device int64 [b]) and their features, with no host sync.  A batch over its
+        capacity is published empty with the buffers' flag raised; the caller reads the flag."""
+        buf = self._buffers(ids.numel())
+        first = self.next_sample                       # fresh walk randomness for every item drawn, like the reference
+        self.next_sample += buf.B
+        sample_pairs(self, buf, first, ids)
+        buf.posenc()
         return buf
-
-    posenc = LoadBalanceGraphDataset.posenc
 
 
 class GraphClassificationDatasetLabeled(_LabeledBase):
@@ -359,23 +337,15 @@ class GraphClassificationDatasetLabeled(_LabeledBase):
         self.num_classes = int(self.labels.max()) + 1                   # dataset.num_labels
         self.length = self.total = len(graphs)
         assert len(self.labels) == self.length
-        # the reference's self.dict (:355): every item is prepared once.  seed = argmax degree (:361, first
-        # maximum), moved to row 0; the relabelled items also form one union CSR (the gccb_graph_set_t layout)
-        self.seeds, self.items, indptr, indices, node_off, edge_off = seed_first_union(graphs)
-        self.sizes = np.array([g.num_nodes for g in graphs], dtype=np.int64)
-        self.nnz = np.array([len(g.indices) for g in graphs], dtype=np.int64)
         self.device = torch.device(device)
         _lib.require_device()
+        # the reference's self.dict (:355): every item is prepared once.  seed = argmax degree (:361, first
+        # maximum), moved to row 0; the relabelled items form one union CSR on the device
+        self.graph_set = DeviceGraphSet(graphs, self.device)
+        self.seeds, self.items = self.graph_set.seeds, self.graph_set.items      # each item's seed and graph
         self.batch_size = int(min(batch_size, self.length))
         self._bufs = {}
-        to = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a)).to(device=self.device, dtype=dt)
-        self.union_indptr, self.union_indices = to(indptr, torch.int64), to(indices, torch.int32)
-        self.node_off_host = node_off
-        self.union_node_off, self.union_edge_off = to(node_off, torch.int64), to(edge_off, torch.int64)
-        self.set_c = _capi.GraphSet(self.union_indptr.data_ptr(), self.union_indices.data_ptr(),
-                                    self.union_node_off.data_ptr(), self.union_edge_off.data_ptr(), self.length)
-        self.labels_dev = to(self.labels, torch.int64)                       # FinetuneEngine's label table
-        self._features = None
+        self.labels_dev = torch.from_numpy(self.labels).to(self.device)      # FinetuneEngine's label table
 
     @staticmethod
     def _load(dataset):
@@ -397,52 +367,19 @@ class GraphClassificationDatasetLabeled(_LabeledBase):
                                   % (dataset, GRAPH_CLASSIFICATION_DSETS))
 
     def _new_buffers(self, B):
-        top = np.sort(self.sizes)[::-1][:B].sum()
-        top_e = np.sort(self.nnz)[::-1][:B].sum()
-        return BatchBuffers(B, int(top) + 8, int(top_e) + 8, self.positional_embedding_size, 64, self.device)
-
-    def _make_batch(self, chunk):
-        buf = self._buffers(len(chunk))
-        fill_whole_graphs(buf, [self.items[i] for i in chunk], view=0)
-        _posenc(buf)
-        buf.check_flags()
-        return BatchedSubgraphs(buf, 0)
+        return self.graph_set.buffers(B, self.positional_embedding_size)
 
     def feature_cache(self):
-        """Positional features of every vertex of the union, [total vertices][P], computed once on first use.  The
-        eigensolver is deterministic, so these are the rows _make_batch computes for a graph in any batch.  Built
-        from batches of consecutive ids, whose rows are the union's rows in order: one device copy per batch."""
-        if self._features is None:
-            P, B = self.positional_embedding_size, self.batch_size
-            no = self.node_off_host
-            cache = torch.empty(int(no[-1]), P, dtype=torch.float32, device=self.device)
-            full = self._buffers(B)
-            ids = torch.arange(self.length, dtype=torch.int64, device=self.device)
-            for a in range(0, self.length, B):
-                b = min(B, self.length - a)
-                buf = full.narrow(b)
-                _lib.check(_lib.get().gccb_gather_graphs(C.byref(self.set_c), _lib.dptr(ids[a:a + b]), C.byref(buf.c),
-                                                         _lib.stream_ptr()), "gccb_gather_graphs")
-                buf.node_off[1].zero_()                # view 1 absent for the eigensolver, as fill_whole_graphs
-                buf.edge_off[1].zero_()
-                buf.node_off[1, b] = -1
-                buf.counters[b:2 * b].zero_()
-                _posenc(buf)
-                cache[no[a]:no[a + b]].copy_(buf.pos[0, :no[a + b] - no[a]])
-            full.check_flags()
-            self._features = cache
-        return self._features
+        """The graph set's feature cache (DeviceGraphSet.feature_cache), built in batches of batch_size graphs."""
+        return self.graph_set.feature_cache(self.positional_embedding_size, self.batch_size)
 
     def device_batch(self, ids):
-        """_make_batch for the graphs `ids` (device int64 [b]) with no host sync: the union gather and the cached
+        """The whole graphs `ids` (device int64 [b]) with no host sync: the union gather and, in view 0, the cached
         features.  The buffers hold the b largest graphs, so a batch never overflows."""
         buf = self._buffers(ids.numel())
-        lib, st = _lib.get(), _lib.stream_ptr()
-        _lib.check(lib.gccb_gather_graphs(C.byref(self.set_c), _lib.dptr(ids), C.byref(buf.c), st),
-                   "gccb_gather_graphs")
-        _lib.check(lib.gccb_gather_features(C.byref(self.set_c), _lib.dptr(ids), C.byref(buf.c), 0,
-                                            _lib.dptr(self.feature_cache()), buf.pos_dim, _lib.dptr(buf.pos), st),
-                   "gccb_gather_features")
+        self.feature_cache()
+        self.graph_set.gather(ids, buf)
+        self.graph_set.gather_features(ids, buf)
         return buf
 
 

@@ -122,7 +122,7 @@ def main():
         if name == "nodes":
             extra = dict(directed_edges=int(ds.graph.indices.numel()), nodes=ds.graph.num_nodes)
         else:
-            extra = dict(mean_vertices=round(float(ds.sizes.mean()), 1))
+            extra = dict(mean_vertices=round(float(ds.graph_set.sizes.mean()), 1))
         with contextlib.redirect_stdout(io.StringIO()):              # the per-step training lines
             r = run(name, ds, a.reps)
         r.update(extra)

@@ -11,7 +11,6 @@ import torch
 
 import train
 from gcc_b200.datasets import labeled
-from gcc_b200.datasets.graph_dataset import LoadBalanceGraphDataset
 
 
 @pytest.mark.parametrize("gpus,want", [
@@ -42,13 +41,14 @@ def _node_dataset():
 def recorded_batches(monkeypatch):
     calls = []
 
-    def sample_batch(ds, first_sample=None, seeds=None, buffers=None, posenc=True):
-        calls.append((id(ds), first_sample, seeds.tolist(), buffers))
-        return buffers
+    def sample_pairs(ds, buf, first_sample, seeds=None):
+        calls.append((id(ds), first_sample, seeds.tolist(), buf))
+        return buf
 
-    monkeypatch.setattr(LoadBalanceGraphDataset, "sample_batch", sample_batch)
+    monkeypatch.setattr(labeled, "sample_pairs", sample_pairs)
     monkeypatch.setattr(labeled.NodeClassificationDatasetLabeled, "_new_buffers",
-                        lambda self, B: types.SimpleNamespace(B=B, flags=torch.zeros(1, dtype=torch.int32)))
+                        lambda self, B: types.SimpleNamespace(B=B, flags=torch.zeros(1, dtype=torch.int32),
+                                                              posenc=lambda: None))
     return calls
 
 
@@ -87,17 +87,20 @@ def test_fold_views_draw_what_fresh_datasets_draw(recorded_batches):
 def test_graph_fold_views_share_the_feature_cache():
     ds = object.__new__(labeled.GraphClassificationDatasetLabeled)
     ds._bufs = {8: "the base's buffers"}
+    ds.positional_embedding_size, ds.batch_size = 32, 8
     built = []
-    ds._features = None
+    gs = ds.graph_set = types.SimpleNamespace(features=None)      # DeviceGraphSet without the device
 
-    def feature_cache():
-        if ds._features is None:
-            built.append(1)
-            ds._features = torch.zeros(3)
-        return ds._features
-    ds.feature_cache = feature_cache
+    def feature_cache(pos_dim, B):
+        if gs.features is None:
+            built.append((pos_dim, B))
+            gs.features = torch.zeros(3)
+        return gs.features
+    gs.feature_cache = feature_cache
     a, b = ds.fold_view(), ds.fold_view()
-    assert len(built) == 1 and a._features is b._features is ds._features
+    assert built == [(32, 8)]                                   # built by the first fold_view, before any fold used it
+    assert a.feature_cache() is b.feature_cache() is ds.feature_cache() is gs.features
+    assert len(built) == 1 and a.graph_set is b.graph_set is gs
     assert a._bufs == {} and b._bufs == {} and a._bufs is not b._bufs
 
 

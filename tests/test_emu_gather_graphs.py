@@ -1,5 +1,5 @@
 """gccb_gather_graphs under the CPU emulator: both views of a whole-graph batch, bit-exact against
-labeled.fill_whole_graphs (the host assembly of the finetune path), on TU-style multigraphs with parallel edges,
+labeled.fill_whole_graphs (the host assembly of a whole-graph batch), on TU-style multigraphs with parallel edges,
 self loops, an isolated vertex and seeds that are not vertex 0; and the capacity contract of the sampler (flag
 raised, batch published empty) for node and edge overflow."""
 import ctypes as C

@@ -295,19 +295,27 @@ def test_engine_on_reference_golden():
 
 def test_feature_cache_matches_per_batch_features():
     """The cached rows are bit-identical to fill_whole_graphs + posenc of the same graphs in shuffled batches of
-    other compositions (and other batch sizes)."""
+    other compositions (and other batch sizes), and so are the rows and eigenvalues of the batches the dataset
+    gives."""
+    from gcc_b200.datasets.labeled import fill_whole_graphs
     ds = _graph_set(batch_size=16)
+    gs = ds.graph_set
     cache = ds.feature_cache().cpu().numpy()
-    no = ds.node_off_host
+    no = gs.node_off_host
     order = np.random.RandomState(2).permutation(len(ds))
     for bs in (16, 7):
         for a in range(0, len(ds), bs):
             chunk = order[a:a + bs]
-            g = ds._make_batch(chunk)
-            buf = g.buffers
-            n = int(buf.node_off[0, buf.B])
-            want = np.concatenate([cache[no[i]:no[i + 1]] for i in chunk])
-            assert buf.pos[0, :n].cpu().numpy().tobytes() == want.tobytes(), (bs, a)
+            b = len(chunk)
+            ref = fill_whole_graphs(gs.buffers(b, 32), [gs.items[i] for i in chunk], view=0)
+            ref.posenc()
+            ref.check_flags()
+            n = int(ref.node_off[0, b])
+            want = ref.pos[0, :n].cpu().numpy().tobytes()
+            assert np.concatenate([cache[no[i]:no[i + 1]] for i in chunk]).tobytes() == want, (bs, a)
+            buf = ds._make_batch(chunk).buffers
+            assert int(buf.node_off[0, b]) == n and buf.pos[0, :n].cpu().numpy().tobytes() == want, (bs, a)
+            assert torch.equal(buf.eigvals[:b], ref.eigvals[:b]), (bs, a)         # the cached eigenvalues too
 
 
 def test_epoch_issues_no_host_sync():
