@@ -15,7 +15,6 @@
 #include "tc_gemm.cuh"
 #ifndef GCCB_EMU
 #include <cuda_bf16.h>
-#include <stdlib.h>
 #endif
 
 namespace gccb {
@@ -120,67 +119,9 @@ nce_loss_kernel(const float* __restrict__ out, int B, int C, int label_mode,
 
 // ---- fused InfoNCE -------------------------------------------------------------------------
 // partial record per (chunk, row): m, s, acc[d]  ->  stride d + 2 floats
-// grid = (nchunks, ceil(B/RB)), block 256; dyn smem: qs[RB][d] | ms[CK][d+1] | ps[RB][CK]
-__global__ void __launch_bounds__(256)
-infonce_partial_kernel(const float* __restrict__ q, const float* __restrict__ mem, int B, int d,
-                       int K, int CK, float invT, float* __restrict__ part) {
-  GCCB_DYN_SMEM(float, smem);
-  float* qs = smem;
-  float* ms = qs + GCCB_NCE_RB * d;
-  float* ps = ms + (size_t)CK * (d + 1);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int i0 = blockIdx.y * GCCB_NCE_RB, j0 = blockIdx.x * CK;
-  const int nk = min(CK, K - j0);
-  for (int idx = tid; idx < GCCB_NCE_RB * d; idx += 256) {
-    int i = i0 + idx / d;
-    qs[idx] = i < B ? q[(size_t)i * d + idx % d] : 0.f;
-  }
-  for (int idx = tid; idx < CK * d; idx += 256) {
-    int j = idx / d, c = idx - j * d;
-    ms[j * (d + 1) + c] = j < nk ? mem[(size_t)(j0 + j) * d + c] : 0.f;
-  }
-  __syncthreads();
-  for (int idx = tid; idx < GCCB_NCE_RB * CK; idx += 256) {
-    int r = idx / CK, j = idx - r * CK;
-    float s = 0.f;
-    for (int c = 0; c < d; ++c) s = fmaf(qs[r * d + c], ms[j * (d + 1) + c], s);
-    ps[idx] = j < nk ? s * invT : -3.0e38f;
-  }
-  __syncthreads();
-  // warp r owns row r: chunk max and sum of exp
-  {
-    const int r = warp;                                   // 8 warps == RB rows
-    float mx = -3.0e38f;
-    for (int j = lane; j < CK; j += 32) mx = fmaxf(mx, ps[r * CK + j]);
-    mx = warp_max(mx);
-    float s = 0.f;
-    for (int j = lane; j < CK; j += 32) {
-      float p = j < nk ? expf(ps[r * CK + j] - mx) : 0.f;
-      ps[r * CK + j] = p;
-      s += p;
-    }
-    s = warp_sum(s);
-    if (lane == 0 && i0 + r < B) {
-      float* rec = part + ((size_t)blockIdx.x * B + i0 + r) * (d + 2);
-      rec[0] = mx;
-      rec[1] = s;
-    }
-  }
-  __syncthreads();
-  for (int idx = tid; idx < GCCB_NCE_RB * d; idx += 256) {
-    int r = idx / d, c = idx - r * d;
-    if (i0 + r >= B) continue;
-    float a = 0.f;
-    for (int j = 0; j < nk; ++j) a = fmaf(ps[r * CK + j], ms[j * (d + 1) + c], a);
-    part[((size_t)blockIdx.x * B + i0 + r) * (d + 2) + 2 + c] = a;
-  }
-}
-
-// merge partials with the positive logit; loss_i, dq_i; stats[0] += loss_i/B, stats[1] += l_pos/B
-// Tiled variant for d in {32, 64, 128, 256}: 32 query rows x CK = 32*KPT keys per CTA (4x fewer
-// passes over the queue than the 8-row kernel), register tiles for both products.  Warp w owns
-// rows 4w..4w+3; lane owns keys lane + 32t (logits) and columns lane + 32u (accumulator).
-// dyn smem: qs[32][d] | ms[CK][d+1] | ps[32][CK].  Same partial-record layout as above.
+// d in {32, 64, 128, 256}: 32 query rows x CK = 32*KPT keys per CTA, register tiles for both products.
+// Warp w owns rows 4w..4w+3; lane owns keys lane + 32t (logits) and columns lane + 32u (accumulator).
+// grid = (nchunks, ceil(B/32)), block 256; dyn smem: qs[32][d] | ms[CK][d+1] | ps[32][CK]
 #define GCCB_NCE_RB2 32
 template <int KPT, int DU>
 __global__ void __launch_bounds__(256)
@@ -272,6 +213,7 @@ infonce_partial_tiled_kernel(const float* __restrict__ q, const float* __restric
   }
 }
 
+// merge partials with the positive logit; loss_i, dq_i; stats[0] += loss_i/B, stats[1] += l_pos/B
 // grid = B, block 128 (threads over d)
 __global__ void __launch_bounds__(128)
 infonce_merge_kernel(const float* __restrict__ q, const float* __restrict__ k,
@@ -421,9 +363,7 @@ static NceTcLayout nce_tc_layout(int B, int d, int K) {
   return L;
 }
 static bool nce_use_tc(int B, int d, int K) {
-  static int env = -1;
-  if (env < 0) { const char* e = getenv("GCCB200_TC"); env = (e && e[0] == '0') ? 0 : 1; }
-  return env && d >= 128 && d % 64 == 0 && K % 64 == 0 && B >= 128;
+  return d >= 128 && K % 64 == 0 && B >= 128;       // d is 128 or 256 here
 }
 
 // one CTA per query row: positive logit (fp32 q.k), row max / sum over [lpos | logits], loss and statistics,
@@ -524,12 +464,9 @@ static int infonce_tc(const float* q, const float* k, const float* memory, int B
 }
 #endif  // !GCCB_EMU
 
-static bool infonce_tiled(int d) { return d == 32 || d == 64 || d == 128 || d == 256; }
-static int infonce_ck(int d) {
-  if (infonce_tiled(d)) return d <= 128 ? 128 : 64;
-  int ck = 16384 / d;
-  return ck < 32 ? 32 : (ck > 256 ? 256 : ck);
-}
+// the encoder widths; the fused head has a tiled kernel for each
+static bool infonce_width(int d) { return d == 32 || d == 64 || d == 128 || d == 256; }
+static int infonce_ck(int d) { return d <= 128 ? 128 : 64; }   // keys per CTA of infonce_partial_tiled_kernel
 
 }  // namespace gccb
 
@@ -573,6 +510,7 @@ extern "C" int gccb_nce_loss(const float* out, int32_t B, int32_t C, int32_t lab
 }
 
 extern "C" size_t gccb_infonce_workspace(int32_t B, int32_t d, int32_t K) {
+  if (!infonce_width(d)) return 0;
   int ck = infonce_ck(d);
   size_t nch = (size_t)(K + ck - 1) / ck;
   size_t simt = nch * (size_t)B * (d + 2) * sizeof(float);
@@ -587,6 +525,10 @@ extern "C" int gccb_infonce_fused(const float* q, const float* k, const float* m
                                   size_t workspace_bytes, gccb_stream_t stream) {
   if (bad_head_args("gccb_infonce_fused", q, k, B, d, K) || !memory || !stats || !dq || !workspace)
     return GCCB_ERR_BADARG;
+  if (!infonce_width(d)) {
+    set_last_error("gccb_infonce_fused: d = %d (need d in {32, 64, 128, 256})", d);
+    return GCCB_ERR_BADARG;
+  }
   if (workspace_bytes < gccb_infonce_workspace(B, d, K)) {
     set_last_error("gccb_infonce_fused: workspace too small");
     return GCCB_ERR_CAPACITY;
@@ -597,27 +539,19 @@ extern "C" int gccb_infonce_fused(const float* q, const float* k, const float* m
 #ifndef GCCB_EMU
   if (nce_use_tc(B, d, K)) return infonce_tc(q, k, memory, B, d, K, T, stats, dq, (char*)workspace, (cudaStream_t)stream);
 #endif
-  if (infonce_tiled(d)) {
-    const size_t smem = ((size_t)GCCB_NCE_RB2 * d + (size_t)ck * (d + 1) + (size_t)GCCB_NCE_RB2 * ck) * 4;
-    dim3 grid(nch, (B + GCCB_NCE_RB2 - 1) / GCCB_NCE_RB2);
+  const size_t smem = ((size_t)GCCB_NCE_RB2 * d + (size_t)ck * (d + 1) + (size_t)GCCB_NCE_RB2 * ck) * 4;
+  dim3 grid(nch, (B + GCCB_NCE_RB2 - 1) / GCCB_NCE_RB2);
 #define GCCB_NCE_TILED(KPT, DU)                                                              \
   do {                                                                                       \
     auto kt = infonce_partial_tiled_kernel<KPT, DU>;                                         \
     gccb::ensure_dyn_smem(kt, smem);                                                         \
     GCCB_LAUNCH(kt, grid, 256, smem, stream, q, memory, B, K, 1.0f / T, (float*)workspace); \
   } while (0)
-    if (d == 32) GCCB_NCE_TILED(4, 1);
-    else if (d == 64) GCCB_NCE_TILED(4, 2);
-    else if (d == 128) GCCB_NCE_TILED(4, 4);
-    else GCCB_NCE_TILED(2, 8);
+  if (d == 32) GCCB_NCE_TILED(4, 1);
+  else if (d == 64) GCCB_NCE_TILED(4, 2);
+  else if (d == 128) GCCB_NCE_TILED(4, 4);
+  else GCCB_NCE_TILED(2, 8);
 #undef GCCB_NCE_TILED
-  } else {
-    const size_t smem = ((size_t)GCCB_NCE_RB * d + (size_t)ck * (d + 1) + (size_t)GCCB_NCE_RB * ck) * 4;
-    auto kp = infonce_partial_kernel;
-    gccb::ensure_dyn_smem(kp, smem);
-    dim3 grid(nch, (B + GCCB_NCE_RB - 1) / GCCB_NCE_RB);
-    GCCB_LAUNCH(kp, grid, 256, smem, stream, q, memory, B, d, K, ck, 1.0f / T, (float*)workspace);
-  }
   GCCB_LAUNCH(infonce_merge_kernel, B, 128, 0, stream, q, k, (const float*)workspace, B, d, nch, 1.0f / T,
               stats, dq);
   return check_launch("gccb_infonce_fused");

@@ -15,10 +15,9 @@ from .. import _capi
 
 def make_cfg(num_layers=5, hidden=64, pos_dim=32, deg_dim=16, max_degree=512, norm=True,
              bn_eps=1e-5, bn_momentum=0.1, norm_eps=1e-5, dropout_p=0.5, tensor_cores=None):
-    """tensor_cores: None = default (on for hidden >= 128 unless GCCB200_TC=0 is set in the environment)."""
-    import os
+    """tensor_cores: None = on for hidden >= 128 (the fp32 SIMT path stays selectable with tensor_cores=0)."""
     if tensor_cores is None:
-        tensor_cores = hidden >= 128 and os.environ.get("GCCB200_TC", "1") != "0"
+        tensor_cores = hidden >= 128
     return _capi.GinCfg(num_layers, hidden, pos_dim, deg_dim, max_degree, int(bool(norm)),
                         bn_eps, bn_momentum, norm_eps, dropout_p, int(bool(tensor_cores)), 0)
 

@@ -333,7 +333,11 @@ int gccb_moco_logits_backward(const float* dout, const float* k, const float* me
 int gccb_nce_loss(const float* out, int32_t B, int32_t C, int32_t label_mode, float* loss,
                   float* dout, gccb_stream_t stream);
 /* fused InfoNCE: loss and dq in one pass over the queue, logits never materialised.
- * stats[0] = loss, stats[1] = mean positive logit ("prob", train.py:394).               */
+ * stats[0] = loss, stats[1] = mean positive logit ("prob", train.py:394).
+ * d must be 32, 64, 128 or 256 (the encoder widths): other widths return GCCB_ERR_BADARG,
+ * and gccb_infonce_workspace returns 0 for them.  d >= 128 with B >= 128 and K a multiple
+ * of 64 runs on the tensor cores (bf16 operands, fp32 softmax); every other shape runs the
+ * fp32 tiled kernel.                                                                     */
 size_t gccb_infonce_workspace(int32_t B, int32_t d, int32_t K);
 int gccb_infonce_fused(const float* q, const float* k, const float* memory, int32_t B,
                        int32_t d, int32_t K, float T, float* stats, float* dq, void* workspace,

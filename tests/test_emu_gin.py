@@ -219,7 +219,7 @@ def test_stash_layout_locates_the_forward_intermediates(monkeypatch):
             np.abs(got - want.numpy()).max()
 
 
-def test_moco_head_and_optimiser_vs_oracle():
+def test_moco_head_fused_at_d32_and_optimiser_vs_oracle():
     Lb = lib()
     rng = np.random.default_rng(0)
     B, d, K, T = 6, 16, 50, 0.07
@@ -239,13 +239,16 @@ def test_moco_head_and_optimiser_vs_oracle():
     dq = np.zeros_like(q)
     assert Lb.gccb_moco_logits_backward(ptr(dout), ptr(k), ptr(mem), B, d, K, T, ptr(dq), None) == 0
     assert np.allclose(dq, dq_o.numpy(), rtol=1e-4, atol=1e-6)
-    # fused
-    stats = np.zeros(2, np.float32); dq2 = np.zeros_like(q)
-    ws = np.zeros(Lb.gccb_infonce_workspace(B, d, K), np.uint8)
-    assert Lb.gccb_infonce_fused(ptr(q), ptr(k), ptr(mem), B, d, K, T, ptr(stats), ptr(dq2), ptr(ws), ws.nbytes, None) == 0
+    # fused, at the encoder width 32: zero columns appended to q, k and the queue leave the loss and dq unchanged
+    dp = 32
+    qp, kp, memp = (np.pad(a, ((0, 0), (0, dp - d))) for a in (q, k, mem))
+    stats = np.zeros(2, np.float32); dq2 = np.zeros_like(qp)
+    ws = np.zeros(Lb.gccb_infonce_workspace(B, dp, K), np.uint8)
+    assert Lb.gccb_infonce_fused(ptr(qp), ptr(kp), ptr(memp), B, dp, K, T, ptr(stats), ptr(dq2), ptr(ws), ws.nbytes,
+                                 None) == 0
     assert np.isclose(stats[0], float(loss_o), rtol=1e-5)
     assert np.isclose(stats[1], out_o[:, 0].mean().item(), rtol=1e-5)
-    assert np.allclose(dq2, dq_o.numpy(), rtol=1e-4, atol=1e-6)
+    assert np.allclose(dq2[:, :d], dq_o.numpy(), rtol=1e-4, atol=1e-6) and not dq2[:, d:].any()
     # label-arange mode + E2E head
     sq = out[:, :B].copy()
     assert Lb.gccb_nce_loss(ptr(sq), B, B, 1, ptr(loss), None, None) == 0
@@ -327,3 +330,19 @@ def test_fused_infonce_tiled_kernel_ragged_shapes(B, d, K):
     assert np.isclose(stats[0], float(loss_o), rtol=2e-5), (stats[0], float(loss_o))
     assert np.isclose(stats[1], out_o[:, 0].mean().item(), rtol=2e-5)
     assert np.allclose(dq, dq_o.numpy(), rtol=2e-4, atol=2e-6), np.abs(dq - dq_o.numpy()).max()
+
+
+def test_fused_infonce_refuses_other_widths():
+    """The fused head has kernels for the encoder widths only: d = 48 is refused with a message and has no
+    workspace size.  The unfused logits keep taking it."""
+    Lb = lib()
+    B, d, K = 4, 48, 40
+    q, k = np.ones((B, d), np.float32), np.ones((B, d), np.float32)
+    mem = np.ones((K, d), np.float32)
+    stats = np.zeros(2, np.float32); dq = np.zeros_like(q); ws = np.zeros(1 << 16, np.uint8)
+    assert Lb.gccb_infonce_workspace(B, d, K) == 0
+    rc = Lb.gccb_infonce_fused(ptr(q), ptr(k), ptr(mem), B, d, K, 0.07, ptr(stats), ptr(dq), ptr(ws), ws.nbytes, None)
+    assert rc == _capi.GCCB_ERR_BADARG
+    assert b"d = 48" in Lb.gccb_last_error()
+    out = np.zeros((B, K + 1), np.float32)
+    assert Lb.gccb_moco_logits(ptr(q), ptr(k), ptr(mem), B, d, K, 0.07, ptr(out), None) == 0

@@ -286,7 +286,7 @@ def test_fused_infonce_real_sizes(B, K, d):
     _lib.check(lib.gccb_infonce_fused(_lib.dptr(q), _lib.dptr(k), _lib.dptr(mem), B, d, K, 0.07, _lib.dptr(stats),
                                       _lib.dptr(dq), _lib.dptr(ws), ws.numel(), _lib.stream_ptr()))
     torch.cuda.synchronize()
-    tc = d >= 128 and B >= 128 and os.environ.get("GCCB200_TC", "1") != "0"      # tensor-core path (moco.cu: nce_use_tc)
+    tc = d >= 128 and B >= 128 and K % 64 == 0      # tensor-core path (moco.cu: nce_use_tc)
     q64 = q.double().requires_grad_(True)
     # tensor-core path: the two big products take bf16 operands -> the oracle rounds q / queue the same way for the
     # negatives (the positive logit stays fp32 in the kernel)
