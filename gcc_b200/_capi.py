@@ -70,6 +70,16 @@ class GatStash(C.Structure):
                                           "dh", "dz", "dout", "sv", "dx0", "dgates", "dy")])
 
 
+EL_LSCC, EL_PLAIN = 0, 1
+EL_ERR_NAMES = {1: "wrong number of tokens", 2: "not an integer", 3: "vertex id out of range",
+                4: "integer overflows int64", 5: "file ends early", 6: "more keys than the key buffer holds"}
+
+
+class EdgelistState(C.Structure):
+    _fields_ = [(n, C.c_int64) for n in ("lines", "n", "m", "edge_lines", "keys")] + \
+               [("first_error", C.c_uint64), ("error_flags", C.c_int32), ("_pad", C.c_int32)]
+
+
 _PROTOS = {
     "gccb_version": (C.c_int, []),
     "gccb_arch": (C.c_int, []),
@@ -141,6 +151,10 @@ _PROTOS = {
     "gccb_prone_propagate_workspace": (C.c_size_t, [C.c_int64, C.c_int32]),
     "gccb_prone_propagate": (C.c_int, [p, p, p, C.c_int64, p, C.c_int32, C.c_double, p, C.c_int32, p, C.c_size_t,
                                        p, p]),
+    "gccb_edgelist_workspace": (C.c_size_t, [C.c_int64]),
+    "gccb_edgelist_begin": (C.c_int, [C.c_int32, p, C.c_size_t, p]),
+    "gccb_edgelist_parse": (C.c_int, [p, C.c_int64, C.c_int32, p, C.c_int64, p, C.c_size_t, p]),
+    "gccb_edgelist_finish": (C.c_int, [C.c_int32, p, p, C.c_size_t, p]),
 }
 
 SYMBOLS = tuple(_PROTOS)

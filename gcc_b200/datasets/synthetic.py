@@ -47,6 +47,36 @@ def from_pairs(src, dst, n, name="graph"):
     return CSRGraph(indptr, d.astype(np.int32), n2, name)
 
 
+def from_keys_device(keys, n, name="graph"):
+    """The cleaning of x2dgl.py:52-62 on directed keys s*n + d that hold both orientations of every edge and no
+    self loop, with torch on the keys' device: tocsr() (duplicates merged into one entry), then remove_nodes
+    (in_degrees == 0) with the remaining vertices kept in order.  Neighbour lists come out ascending.
+    keys: an int64 tensor or a list of them; a list is emptied here, so that its tensors are freed as soon as
+    the de-duplicated copy exists (BASELINE config 5 holds 400M keys)."""
+    import torch
+    if isinstance(keys, list):
+        key = keys[0] if len(keys) == 1 else torch.cat(keys)
+        keys.clear()
+    else:
+        key = keys
+    del keys
+    key = torch.unique(key, sorted=True)
+    s, d = key // n, key % n
+    device = key.device
+    del key
+    deg = torch.bincount(s, minlength=n)
+    del s
+    alive = deg > 0
+    n2 = int(alive.sum())
+    if n2 != n:
+        remap = torch.cumsum(alive.long(), 0) - 1
+        d = remap[d]
+        deg = deg[alive]
+    indptr = torch.zeros(n2 + 1, dtype=torch.int64, device=device)
+    torch.cumsum(deg, 0, out=indptr[1:])
+    return CSRGraph(indptr, d.to(torch.int32), n2, name)
+
+
 def erdos_renyi(n=1000, n_pairs=5000, seed=0):
     """C1: ER G(n, pairs)."""
     rng = np.random.default_rng(seed)
@@ -137,19 +167,7 @@ def chung_lu_device(n=1_000_000, n_pairs=20_000_000, exponent=0.5, seed=0, devic
         keys.append(src * n + dst)
         keys.append(dst * n + src)
         left -= c
-    key = torch.unique(torch.cat(keys), sorted=True)
-    del keys
-    s, d = key // n, key % n
-    deg = torch.bincount(s, minlength=n)
-    alive = deg > 0
-    n2 = int(alive.sum())
-    if n2 != n:
-        remap = torch.cumsum(alive.long(), 0) - 1
-        d = remap[d]
-        deg = deg[alive]
-    indptr = torch.zeros(n2 + 1, dtype=torch.int64, device=device)
-    torch.cumsum(deg, 0, out=indptr[1:])
-    return CSRGraph(indptr, d.to(torch.int32), n2, "chunglu_dev_n%d_p%d" % (n, n_pairs))
+    return from_keys_device(keys, n, "chunglu_dev_n%d_p%d" % (n, n_pairs))
 
 
 def rmat_device(scale=24, n_pairs=200_000_000, abcd=(0.57, 0.19, 0.19, 0.05), seed=0, device="cuda"):
@@ -179,17 +197,4 @@ def rmat_device(scale=24, n_pairs=200_000_000, abcd=(0.57, 0.19, 0.19, 0.05), se
         keys.append(src * n + dst)
         keys.append(dst * n + src)
         left -= m
-    key = torch.unique(torch.cat(keys), sorted=True)
-    del keys
-    s, d = key // n, key % n
-    del key
-    deg = torch.bincount(s, minlength=n)
-    del s
-    alive = deg > 0
-    n2 = int(alive.sum())
-    remap = torch.cumsum(alive.long(), 0) - 1
-    d = remap[d].to(torch.int32)
-    deg = deg[alive]
-    indptr = torch.zeros(n2 + 1, dtype=torch.int64, device=device)
-    torch.cumsum(deg, 0, out=indptr[1:])
-    return CSRGraph(indptr, d, n2, "rmat_dev_s%d_p%d" % (scale, n_pairs))
+    return from_keys_device(keys, n, "rmat_dev_s%d_p%d" % (scale, n_pairs))

@@ -426,6 +426,50 @@ int gccb_clip_value_adagrad(float* p, const float* g, float* sum, int64_t n, con
 int gccb_gather_features(const gccb_graph_set_t* set, const int64_t* graph_ids, const gccb_batch_t* batch,
                          int32_t view, const float* cache, int32_t pos_dim, float* pos, gccb_stream_t stream);
 
+/* ---- corpus builder: edge-list text -> directed keys (csrc/edgelist.cu) ------------------------------------
+ * Replaces the per-line loop of yuxiao_kdd17_graph_to_dgl (gcc/utils/x2dgl.py:28-47).  The caller streams a file
+ * through gccb_edgelist_parse in chunks of whole lines (each chunk ends at a '\n', except the file's last one) and
+ * gets, in file line order, two int64 keys per edge line that is not a self loop: min*n + max, then max*n + min.
+ * Tokens are runs of characters other than ' ', '\t', '\r'; an integer token is -?[0-9]+ within int64.
+ *   GCCB_EL_LSCC:  line 0's second token is n, lines 1..n are skipped, line n+1's second token is m, then m lines
+ *                  of exactly three integers "u v w" (w is ignored; an overflow of w is not an error); later lines
+ *                  are ignored.  0 <= n < 2^31.  Keys use the multiplier n.
+ *   GCCB_EL_PLAIN: every line "u v [anything]"; blank lines and lines whose first token starts with '#' or '%' are
+ *                  skipped.  n = 1 + the largest id of an edge that is not a self loop.  The parse uses the
+ *                  multiplier 2^31 (ids must be below it); gccb_edgelist_finish rewrites the keys to s*n + d.
+ * An id of an edge that is not a self loop must lie in [0, n).  Errors never fault: state.first_error holds
+ * (line << 4) | kind of the offending line with the smallest 0-based index, error_flags the OR of 1 << kind.
+ * The state lives at the start of the workspace; the caller reads it back after gccb_edgelist_finish.
+ * Deterministic: no key's slot depends on an atomic.                                                      */
+#define GCCB_EL_LSCC 0
+#define GCCB_EL_PLAIN 1
+#define GCCB_EL_ERR_TOKENS 1    /* wrong token count (.lscc edge line != 3, header < 2, plain < 2)        */
+#define GCCB_EL_ERR_CHAR 2      /* a read token is not -?[0-9]+                                             */
+#define GCCB_EL_ERR_RANGE 3     /* id < 0 or >= n (plain: >= 2^31); header n or m < 0 or >= 2^31           */
+#define GCCB_EL_ERR_OVERFLOW 4  /* an id outside int64                                                      */
+#define GCCB_EL_ERR_SHORT 5     /* .lscc: the header or fewer than m edge lines (line = the first missing)  */
+#define GCCB_EL_ERR_CAPACITY 6  /* more keys than keys_cap                                                  */
+typedef struct {
+  int64_t lines;          /* lines parsed so far                                                    */
+  int64_t n;              /* .lscc: header n (-1 unread, -2 bad); plain: 1 + largest id so far     */
+  int64_t m;              /* .lscc: header m (-1 unread, -2 bad)                                    */
+  int64_t edge_lines;     /* edge lines read, self loops included (.lscc: at most m)                */
+  int64_t keys;           /* keys written                                                           */
+  uint64_t first_error;   /* (line << 4) | GCCB_EL_ERR_*; all ones = none                           */
+  int32_t error_flags;
+  int32_t _pad;
+} gccb_edgelist_state_t;
+/* workspace for chunks of up to chunk_bytes bytes: about 8 * chunk_bytes (a 64-bit offset per possible line) */
+size_t gccb_edgelist_workspace(int64_t chunk_bytes);
+/* resets the state for a new file */
+int gccb_edgelist_begin(int32_t format, void* workspace, size_t workspace_bytes, gccb_stream_t stream);
+/* one chunk of nbytes bytes of device text; keys: [keys_cap] output of the whole file, appended at state.keys */
+int gccb_edgelist_parse(const char* text, int64_t nbytes, int32_t format, int64_t* keys, int64_t keys_cap,
+                        void* workspace, size_t workspace_bytes, gccb_stream_t stream);
+/* after the last chunk: .lscc records missing header or edge lines; plain rewrites the keys to s*n + d */
+int gccb_edgelist_finish(int32_t format, int64_t* keys, void* workspace, size_t workspace_bytes,
+                         gccb_stream_t stream);
+
 /* ---- tensor-core contraction (wgmma + TMA; csrc/tc_gemm.cu) ---------------------------------------
  * The dense products of the path at hidden >= 128 (BASELINE config 4): the GIN MLP's Linear layers
  * (gcc/models/gin.py:107-116) with the BatchNorm column statistics of :115 fused into the epilogue,
