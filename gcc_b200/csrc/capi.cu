@@ -77,6 +77,20 @@ extern "C" unsigned long long gccb_launch_count(void) { return gccb::g_launch_co
 
 extern "C" const char* gccb_last_error(void) { return gccb::g_err; }
 
+#ifdef GCCB_EMU
+// CPU emulator build only (the fiber emulator of the kernel-logic tests): counts[0..1] = programmatic launches and
+// launches in which a thread returned without pdl_wait(), both since the last call; returns the first offending
+// kernel's name ("" if none) and clears the log
+extern "C" const char* gccb_emu_pdl_log(unsigned long long* counts) {
+  gccb::EmuPdlLog& g = gccb::emu_pdl_log;
+  counts[0] = g.launches;
+  counts[1] = g.unwaited;
+  const char* first = g.first_bad;
+  g = gccb::EmuPdlLog();
+  return first;
+}
+#endif
+
 extern "C" int gccb_arch(void) {
   int dev = 0, major = 0, minor = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) {

@@ -15,6 +15,43 @@ namespace gccb { extern unsigned long long g_launch_count; }
 #undef GCCB_LAUNCH
 #define GCCB_LAUNCH(kern, grid, block, smem, stream, ...) \
   (++gccb::g_launch_count, emu::launch(dim3(grid), dim3(block), (size_t)(smem), [=]() { kern(__VA_ARGS__); }))
+namespace gccb {
+// Programmatic launches under the emulator (GCCB_LAUNCH_PDL): how many ran, in how many some thread returned without
+// calling pdl_wait(), and the first offending kernel's name as the launch spelt it (read by gccb_emu_pdl_log).
+struct EmuPdlLog {
+  unsigned long long launches = 0, unwaited = 0;
+  const char* first_bad = "";
+};
+inline EmuPdlLog emu_pdl_log;
+inline bool emu_pdl_launch = false;        // a GCCB_LAUNCH_PDL kernel is running
+inline bool emu_pdl_violation = false;     // ... and one of its threads returned without waiting
+inline std::vector<char> emu_pdl_waited;   // per thread of the running block: pdl_wait() called
+
+// blocks run one after another, each thread on its own fiber: only whether the wait was called is recorded
+inline void pdl_wait() {
+  if (emu_pdl_launch) emu_pdl_waited[emu::C().cur] = 1;
+}
+template <class F>
+inline void emu_launch_pdl(const char* name, dim3 grid, dim3 block, size_t smem, F kernel_call) {
+  emu_pdl_launch = true;
+  emu_pdl_violation = false;
+  emu_pdl_waited.assign((size_t)block.x * block.y * block.z, 0);
+  emu::launch(grid, block, smem, [=]() {
+    const int t = emu::C().cur;
+    emu_pdl_waited[t] = 0;
+    kernel_call();
+    if (!emu_pdl_waited[t]) emu_pdl_violation = true;
+  });
+  emu_pdl_launch = false;
+  emu_pdl_log.launches++;
+  emu_pdl_log.unwaited += emu_pdl_violation;
+  if (emu_pdl_violation && !*emu_pdl_log.first_bad) emu_pdl_log.first_bad = name;
+}
+}  // namespace gccb
+// runs like GCCB_LAUNCH and logs whether every thread of every block called pdl_wait() before it returned
+#define GCCB_LAUNCH_PDL(kern, grid, block, smem, stream, ...)                                                        \
+  (++gccb::g_launch_count,                                                                                          \
+   gccb::emu_launch_pdl(#kern, dim3(grid), dim3(block), (size_t)(smem), [=]() { kern(__VA_ARGS__); }))
 #else
 #include <cuda_runtime.h>
 #define GCCB_DYN_SMEM(type, name)                                   \
@@ -23,6 +60,38 @@ namespace gccb { extern unsigned long long g_launch_count; }
 namespace gccb { extern unsigned long long g_launch_count; }
 #define GCCB_LAUNCH(kern, grid, block, smem, stream, ...) \
   (++gccb::g_launch_count, kern<<<(grid), (block), (smem), (cudaStream_t)(stream)>>>(__VA_ARGS__))
+
+// Programmatic dependent launch (sm_90).  A kernel launched with GCCB_LAUNCH_PDL becomes pending as soon as every
+// CTA of the kernel before it on the stream has exited, before that kernel's completion has been processed, so its
+// CTAs take SM slots as the predecessor's last ones retire instead of leaving them to the data path's queued CTAs.
+// A kernel launched this way calls pdl_wait() first, before any global load or store and before any return: it
+// blocks until the predecessor has completed and its writes are visible.  Ordering is transitive only if every
+// kernel of the chain waits before it can complete.  No kernel triggers its dependents early
+// (griddepcontrol.launch_dependents): a successor pending while its predecessor still runs holds SM slots while it
+// waits, which starved the data path and made the C2 step 4 % slower (DESIGN.md 7).
+// Under an ordinary launch pdl_wait() does nothing: kernels shared with other callers call it unconditionally.
+namespace gccb {
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+
+template <class... KArgs, class... Args>
+inline void launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
+                       Args&&... args) {
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid;
+  cfg.blockDim = block;
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = stream;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  cudaLaunchKernelEx(&cfg, kern, static_cast<Args&&>(args)...);   // a failure is left for check_launch
+}
+}  // namespace gccb
+#define GCCB_LAUNCH_PDL(kern, grid, block, smem, stream, ...) \
+  (++gccb::g_launch_count,                                    \
+   gccb::launch_pdl(kern, dim3(grid), dim3(block), (size_t)(smem), (cudaStream_t)(stream), __VA_ARGS__))
 #endif
 
 #ifndef GCCB_EMU

@@ -1039,7 +1039,7 @@ static int gat_run_forward(const GatArgs& a, float* feat) {
   cudaMemsetAsync(cs, 0, K * BH * sizeof(float), (cudaStream_t)a.stream);
   const int tgrid = tile_grid(cap), rgrid = row_grid(cap), ggrid = (B + GAT_GB - 1) / GAT_GB;
   GCCB_LAUNCH(gin_build_x0_kernel, tgrid, 256, 0, a.stream, gin_input_dims(d), node_off_v, B,
-              a.pos + (size_t)a.view * cap * d.P, sub_deg, graph_id, P + a.lay.emb, x0);
+              a.pos + (size_t)a.view * cap * d.P, sub_deg, graph_id, P + a.lay.emb, x0, (double*)nullptr, (int64_t)0);
   for (int l = 0; l < d.L; ++l) {
     float* z = (float*)(acts + al.z[l]);
     float* att = (float*)(acts + al.att[l]);

@@ -25,13 +25,17 @@ gin_pool_predict_bwd_kernel(GinDims d, const int32_t* __restrict__ node_off_v, i
                             const float* __restrict__ score, const float* __restrict__ dfeat,
                             uint64_t drop_key, uint64_t drop_step, int drop_layer_base,
                             uint32_t keep_thresh, int DW, float* __restrict__ dS,
-                            float* __restrict__ dpool) {
+                            float* __restrict__ dpool, double* __restrict__ zero, int n_zero) {
   // GCCB_GPB graphs per CTA, like the forward heads: every head weight is read once for all of them
   constexpr int G = GCCB_GPB;
   __shared__ float ds[G][H];
   __shared__ float dsl[G][H];
   const int g0 = blockIdx.x * G, tid = threadIdx.x, lane = tid & 31;
   const int ng = min(G, B - g0);
+  pdl_wait();
+  // the BatchNorm-backward reductions of this call (SIMT path; the tensor-core path passes none): first written by
+  // gin_bwd_dh_kernel, last read on the side stream of the previous call, which the caller joined before this one
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_zero; i += gridDim.x * blockDim.x) zero[i] = 0.0;
   if (node_off_v[B] < 0) return;
   // F.normalize backward: y = x / max(||x||, eps) -- one warp per graph
   for (int gi = tid >> 5; gi < G; gi += 8) {
@@ -104,6 +108,7 @@ gin_pred_wgrad_kernel(GinDims d, int B, gccb_gin_layout_t lay, const float* __re
   const int l = blockIdx.y, H = d.H;
   const int inf = l == 0 ? d.din : H;
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  pdl_wait();
   if (idx < H * inf) {
     const int o = idx / inf, k = idx - o * inf;
     float s = 0.f;
@@ -151,6 +156,7 @@ gin_bwd_dh_kernel(const int32_t* __restrict__ node_off_v, int B, const int32_t* 
   __shared__ float red[BNB ? 9 * 2 * W : 1];         // [8 warps + hub rows][sum g4 | sum g4*yhat][W]
   __shared__ int hub_rows[GCCB_HUB_QUEUE];
   __shared__ int n_hub;
+  pdl_wait();
   const int N = node_off_v[B];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   constexpr int V4 = W / 4, PERV = (V4 + 31) / 32;
@@ -297,6 +303,7 @@ gin_bwd_reduce_kernel(const int32_t* __restrict__ node_off_v, int B,
   __shared__ float coef_a[4 * H];
   __shared__ float coef_b[4 * H];
   __shared__ float red[2 * 1024];
+  pdl_wait();
   const int N = node_off_v[B];
   const int tid = threadIdx.x;
   bn_prepare(sums_a, N, H, ga, bea, bn_eps, coef_a, coef_a + H, coef_a + 2 * H, coef_a + 3 * H, nullptr, false, false, 0.f);
@@ -402,6 +409,7 @@ gin_bwd_gemm2_kernel(const int32_t* __restrict__ node_off_v, int B, const float*
   float* red = Ws + GCCB_KC * (H + 4);
   float* coef = red + 2 * 16 * H;            // 3 bundles of 4H: bn1 | bn_a | bn_b
   float* rmean = coef + 12 * H;              // m_g4 | m_g4y | m_g3 | m_g3z   (4H)
+  pdl_wait();
   const int N = node_off_v[B];
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
   using TC = TileCols<H>;
@@ -478,6 +486,7 @@ gin_bwd_gemm1_kernel(const int32_t* __restrict__ node_off_v, int B, const float*
   float* Ws = As + GCCB_TILE_ROWS * LDA;
   float* coef = Ws + GCCB_KC * (KIN + 4);
   float* rmean = coef + 4 * H;
+  pdl_wait();
   const int N = node_off_v[B];
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
   using TC = TileCols<KIN>;
@@ -530,6 +539,7 @@ gin_wgrad_kernel(const int32_t* __restrict__ node_off_v, int B, int H, int KQ,
   __shared__ float Ps[GCCB_TILE_ROWS][65];
   __shared__ float Qs[GCCB_TILE_ROWS][65];
   __shared__ float qsc[64], qsh[64];
+  pdl_wait();
   const int N = node_off_v[B];
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
   const int kblocks = (KQ + 63) / 64;
@@ -613,6 +623,7 @@ gin_wgrad_reduce_kernel(int H, int KQ, int in_features, const float* __restrict_
                         float* __restrict__ gw, float* __restrict__ gb) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   const size_t stride = (size_t)H * KQ + H;
+  pdl_wait();
   if (idx < H * KQ) {
     const int o = idx / KQ, k = idx - o * KQ;
     if (k < in_features) {
@@ -633,6 +644,7 @@ gin_wgrad_reduce_kernel(int H, int KQ, int in_features, const float* __restrict_
 // BN affine gradients: d gamma = sum g*xhat (red[1]), d beta = sum g (red[0])
 __global__ void gin_bn_grads_kernel(int H, const double* __restrict__ red, float* __restrict__ gw,
                                     float* __restrict__ gb) {
+  pdl_wait();
   int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c < H) { gb[c] += (float)red[c]; gw[c] += (float)red[H + c]; }
 }
@@ -644,6 +656,7 @@ gin_bwd_emb_kernel(GinDims d, const int32_t* __restrict__ node_off_v, int B,
                    const int32_t* __restrict__ sub_deg, const float* __restrict__ dx0,
                    float* __restrict__ gemb) {
   GCCB_DYN_SMEM(float, hist);                // [(maxdeg+1)][D]
+  pdl_wait();
   const int N = node_off_v[B];
   const int cells = (d.maxdeg + 1) * d.D;
   for (int i = threadIdx.x; i < cells; i += blockDim.x) hist[i] = 0.f;
@@ -725,10 +738,11 @@ static int run_backward(const BwdArgs& a) {
 #else
   gccb_stream_t side = a.stream, side1 = a.stream;
 #endif
-  cudaMemsetAsync(red, 0, (size_t)(d.L - 1) * 3 * 2 * H * sizeof(double), (cudaStream_t)a.stream);
+  // Every kernel here is a programmatic dependent of the one before it on its stream (common.cuh); the heads'
+  // backward zeroes the BatchNorm-backward reductions, so that no memset node breaks the chain.
   auto kpb = gin_pool_predict_bwd_kernel<H>;
-  GCCB_LAUNCH(kpb, (B + GCCB_GPB - 1) / GCCB_GPB, 256, 0, a.stream, d, node_off_v, B, P, a.lay, (const float*)(a.acts + a.al.score),
-              a.dfeat, a.drop_key, a.drop_step, a.drop_base, keep, DW, dS, dpool);
+  GCCB_LAUNCH_PDL(kpb, (B + GCCB_GPB - 1) / GCCB_GPB, 256, 0, a.stream, d, node_off_v, B, P, a.lay, (const float*)(a.acts + a.al.score),
+              a.dfeat, a.drop_key, a.drop_step, a.drop_base, keep, DW, dS, dpool, red, (d.L - 1) * 3 * 2 * H);
 #ifndef GCCB_EMU
   cudaEventRecord(ev_head, main_s);
   cudaStreamWaitEvent((cudaStream_t)side, ev_head, 0);
@@ -736,7 +750,7 @@ static int run_backward(const BwdArgs& a) {
   {
     int maxout = H * (d.din > H ? d.din : H) + H;
     dim3 gr((maxout + 255) / 256, d.L);
-    GCCB_LAUNCH(gin_pred_wgrad_kernel, gr, 256, 0, side, d, B, a.lay, (const float*)dS,
+    GCCB_LAUNCH_PDL(gin_pred_wgrad_kernel, gr, 256, 0, side, d, B, a.lay, (const float*)dS,
                 (const float*)(a.acts + a.al.pooled), a.al.PW, G);
   }
   for (int l = d.L - 2; l >= 0; --l) {
@@ -755,11 +769,11 @@ static int run_backward(const BwdArgs& a) {
     // dh_j = dpool_j broadcast + (I + A) da_{j}   (da of the layer above; none for the top)
     // and BN_b's backward reduction (rB) of this layer
     auto kdh = gin_bwd_dh_kernel<H, true>;
-    GCCB_LAUNCH(kdh, (tiles < 1184 ? tiles : 1184), 256, 0, a.stream, node_off_v, B, indptr, indices, graph_id,
+    GCCB_LAUNCH_PDL(kdh, (tiles < 1184 ? tiles : 1184), 256, 0, a.stream, node_off_v, B, indptr, indices, graph_id,
                 (const float*)(dpool + (size_t)j * B * DW), DW, (const float*)da, j < d.L - 1 ? 1 : 0, dh, z2, sa,
                 P + a.lay.bna_w[l], P + a.lay.bna_b[l], sb, P + a.lay.bnb_w[l], P + a.lay.bnb_b[l], d.bn_eps, rB);
     auto kred = gin_bwd_reduce_kernel<H>;
-    GCCB_LAUNCH(kred, grid, 256, 0, a.stream, node_off_v, B, z2, (const float*)dh, sa, P + a.lay.bna_w[l],
+    GCCB_LAUNCH_PDL(kred, grid, 256, 0, a.stream, node_off_v, B, z2, (const float*)dh, sa, P + a.lay.bna_w[l],
                 P + a.lay.bna_b[l], sb, P + a.lay.bnb_w[l], P + a.lay.bnb_b[l], d.bn_eps,
                 (const double*)rB, rA);
 #ifndef GCCB_EMU
@@ -769,7 +783,7 @@ static int run_backward(const BwdArgs& a) {
       auto k = gin_bwd_gemm2_kernel<H>;
       size_t sm = ((size_t)GCCB_TILE_ROWS * (H + 1) + (size_t)GCCB_KC * (H + 4) + 2 * 16 * H + 16 * H) * 4;
       gccb::ensure_dyn_smem(k, sm);
-      GCCB_LAUNCH(k, grid, 256, sm, a.stream, node_off_v, B, z1, z2, (const float*)dh, s1, P + a.lay.bn1_w[l],
+      GCCB_LAUNCH_PDL(k, grid, 256, sm, a.stream, node_off_v, B, z1, z2, (const float*)dh, s1, P + a.lay.bn1_w[l],
                   P + a.lay.bn1_b[l], sa, P + a.lay.bna_w[l], P + a.lay.bna_b[l], sb, P + a.lay.bnb_w[l],
                   P + a.lay.bnb_b[l], d.bn_eps, (const double*)rB, (const double*)rA, P + a.lay.w2[l], dz2,
                   g1, r1);
@@ -782,29 +796,29 @@ static int run_backward(const BwdArgs& a) {
     // (x1 = relu(bn1(z1))) and the three BatchNorm affine gradients
     {
       dim3 gr(GCCB_WG_CHUNKS, ((H + 63) / 64) * ((H + 63) / 64));
-      GCCB_LAUNCH(gin_wgrad_kernel, gr, 256, 0, side, node_off_v, B, H, H, (const float*)dz2, z1, s1,
+      GCCB_LAUNCH_PDL(gin_wgrad_kernel, gr, 256, 0, side, node_off_v, B, H, H, (const float*)dz2, z1, s1,
                   P + a.lay.bn1_w[l], P + a.lay.bn1_b[l], d.bn_eps, part);
-      GCCB_LAUNCH(gin_wgrad_reduce_kernel, (H * H + H + 255) / 256, 256, 0, side, H, H, H,
+      GCCB_LAUNCH_PDL(gin_wgrad_reduce_kernel, (H * H + H + 255) / 256, 256, 0, side, H, H, H,
                   (const float*)part, G + a.lay.w2[l], G + a.lay.b2[l]);
     }
-    GCCB_LAUNCH(gin_bn_grads_kernel, (H + 127) / 128, 128, 0, side, H, (const double*)rB,
+    GCCB_LAUNCH_PDL(gin_bn_grads_kernel, (H + 127) / 128, 128, 0, side, H, (const double*)rB,
                 G + a.lay.bnb_w[l], G + a.lay.bnb_b[l]);
-    GCCB_LAUNCH(gin_bn_grads_kernel, (H + 127) / 128, 128, 0, side, H, (const double*)rA,
+    GCCB_LAUNCH_PDL(gin_bn_grads_kernel, (H + 127) / 128, 128, 0, side, H, (const double*)rA,
                 G + a.lay.bna_w[l], G + a.lay.bna_b[l]);
-    GCCB_LAUNCH(gin_bn_grads_kernel, (H + 127) / 128, 128, 0, side, H, (const double*)r1,
+    GCCB_LAUNCH_PDL(gin_bn_grads_kernel, (H + 127) / 128, 128, 0, side, H, (const double*)r1,
                 G + a.lay.bn1_w[l], G + a.lay.bn1_b[l]);
     const int KQ1 = gin_in_width(d, l), inf = gin_in_features(d, l);
     if (l == 0) {
       auto k = gin_bwd_gemm1_kernel<GCCB_DINP, H>;
       size_t sm = ((size_t)GCCB_TILE_ROWS * (H + 1) + (size_t)GCCB_KC * (GCCB_DINP + 4) + 6 * H) * 4;
       gccb::ensure_dyn_smem(k, sm);
-      GCCB_LAUNCH(k, grid, 256, sm, a.stream, node_off_v, B, z1, g1, s1, P + a.lay.bn1_w[l], P + a.lay.bn1_b[l],
+      GCCB_LAUNCH_PDL(k, grid, 256, sm, a.stream, node_off_v, B, z1, g1, s1, P + a.lay.bn1_w[l], P + a.lay.bn1_b[l],
                   d.bn_eps, (const double*)r1, P + a.lay.w1[l], inf, da);
     } else {
       auto k = gin_bwd_gemm1_kernel<H, H>;
       size_t sm = ((size_t)GCCB_TILE_ROWS * (H + 1) + (size_t)GCCB_KC * (H + 4) + 6 * H) * 4;
       gccb::ensure_dyn_smem(k, sm);
-      GCCB_LAUNCH(k, grid, 256, sm, a.stream, node_off_v, B, z1, g1, s1, P + a.lay.bn1_w[l], P + a.lay.bn1_b[l],
+      GCCB_LAUNCH_PDL(k, grid, 256, sm, a.stream, node_off_v, B, z1, g1, s1, P + a.lay.bn1_w[l], P + a.lay.bn1_b[l],
                   d.bn_eps, (const double*)r1, P + a.lay.w1[l], inf, da);
     }
 #ifndef GCCB_EMU
@@ -814,9 +828,9 @@ static int run_backward(const BwdArgs& a) {
     // second side stream, once GEMM1 has turned g1 into dz1: dW1 = dz1^T a
     {
       dim3 gr1(GCCB_WG_CHUNKS, ((H + 63) / 64) * ((KQ1 + 63) / 64));
-      GCCB_LAUNCH(gin_wgrad_kernel, gr1, 256, 0, side1, node_off_v, B, H, KQ1, (const float*)g1, a_l,
+      GCCB_LAUNCH_PDL(gin_wgrad_kernel, gr1, 256, 0, side1, node_off_v, B, H, KQ1, (const float*)g1, a_l,
                   (const double*)nullptr, (const float*)nullptr, (const float*)nullptr, d.bn_eps, part1);
-      GCCB_LAUNCH(gin_wgrad_reduce_kernel, (H * KQ1 + H + 255) / 256, 256, 0, side1, H, KQ1, inf,
+      GCCB_LAUNCH_PDL(gin_wgrad_reduce_kernel, (H * KQ1 + H + 255) / 256, 256, 0, side1, H, KQ1, inf,
                   (const float*)part1, G + a.lay.w1[l], G + a.lay.b1[l]);
     }
 #ifndef GCCB_EMU
@@ -827,13 +841,13 @@ static int run_backward(const BwdArgs& a) {
   }
   // layer-0 input gradient -> degree embedding
   auto kdh0 = gin_bwd_dh_kernel<GCCB_DINP, false>;
-  GCCB_LAUNCH(kdh0, (tiles < 1184 ? tiles : 1184), 256, 0, a.stream, node_off_v, B, indptr, indices, graph_id, (const float*)dpool, DW,
+  GCCB_LAUNCH_PDL(kdh0, (tiles < 1184 ? tiles : 1184), 256, 0, a.stream, node_off_v, B, indptr, indices, graph_id, (const float*)dpool, DW,
               (const float*)da, 1, dh, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0.f, nullptr);
   {
     size_t sm = (size_t)(d.maxdeg + 1) * d.D * sizeof(float);
     auto k = gin_bwd_emb_kernel;
     gccb::ensure_dyn_smem(k, sm);
-    GCCB_LAUNCH(k, 64, 256, sm, a.stream, d, node_off_v, B, sub_deg, (const float*)dh, G + a.lay.emb);
+    GCCB_LAUNCH_PDL(k, 64, 256, sm, a.stream, d, node_off_v, B, sub_deg, (const float*)dh, G + a.lay.emb);
   }
 #ifndef GCCB_EMU
   cudaEventRecord(ev_join, (cudaStream_t)side1);
@@ -1069,7 +1083,7 @@ static int run_backward_tc(const BwdArgs& a) {
   cudaMemsetAsync(red, 0, (size_t)(d.L - 1) * 3 * 2 * H * sizeof(double), main_s);
   auto kpb = gin_pool_predict_bwd_kernel<H>;
   GCCB_LAUNCH(kpb, (B + GCCB_GPB - 1) / GCCB_GPB, 256, 0, a.stream, d, node_off_v, B, P, a.lay, (const float*)(a.acts + a.al.score),
-              a.dfeat, a.drop_key, a.drop_step, a.drop_base, keep, DW, dS, dpool);
+              a.dfeat, a.drop_key, a.drop_step, a.drop_base, keep, DW, dS, dpool, (double*)nullptr, 0);
   cudaEventRecord(ev_head, main_s);
   cudaStreamWaitEvent(side, ev_head, 0);
   {

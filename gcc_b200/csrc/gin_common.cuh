@@ -415,7 +415,8 @@ __device__ __forceinline__ void tile_colstats(const float (&v)[4][TileCols<NOUT>
 __global__ void __launch_bounds__(256)
 gin_build_x0_kernel(GinDims d, const int32_t* __restrict__ node_off_v, int B, const float* __restrict__ pos,
                     const int32_t* __restrict__ sub_deg, const int32_t* __restrict__ graph_id,
-                    const float* __restrict__ emb, float* __restrict__ x0);
+                    const float* __restrict__ emb, float* __restrict__ x0, double* __restrict__ zero,
+                    int64_t n_zero);
 __global__ void __launch_bounds__(256)
 gin_wgrad_kernel(const int32_t* __restrict__ node_off_v, int B, int H, int KQ, const float* __restrict__ P,
                  const float* __restrict__ Q, const double* __restrict__ q_sums, const float* __restrict__ q_gamma,

@@ -28,7 +28,12 @@ __global__ void __launch_bounds__(256)
 gin_build_x0_kernel(GinDims d, const int32_t* __restrict__ node_off_v, int B,
                     const float* __restrict__ pos, const int32_t* __restrict__ sub_deg,
                     const int32_t* __restrict__ graph_id, const float* __restrict__ emb,
-                    float* __restrict__ x0) {
+                    float* __restrict__ x0, double* __restrict__ zero, int64_t n_zero) {
+  pdl_wait();
+  // the BatchNorm statistics and pooling accumulators of this forward (SIMT path; other callers pass none): their
+  // first writer is the next kernel, and the previous forward's last readers are behind the wait
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_zero; i += (int64_t)gridDim.x * blockDim.x)
+    zero[i] = 0.0;
   const int N = node_off_v[B];
   const int total = N * GCCB_DINP;
   for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += gridDim.x * blockDim.x) {
@@ -91,6 +96,7 @@ gin_agg_gemm1_kernel(const int32_t* __restrict__ node_off_v, int B, const int32_
   __shared__ int n_hub;
   static_assert(8 * KIN <= 2 * 16 * H, "hub scratch must fit in the statistics scratch");
   static_assert(!BN_IN || KIN == H, "the BatchNorm tail is applied to a hidden-width input");
+  pdl_wait();
   const int N = node_off_v[B];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int tx = tid & 15, ty = tid >> 4;
@@ -195,6 +201,7 @@ gin_bn_gemm2_kernel(const int32_t* __restrict__ node_off_v, int B, const float* 
   float* Ws = As + GCCB_TILE_ROWS * LDA;
   float* red = Ws + GCCB_KC * (H + 4);
   float* coef = red + 2 * 16 * H;            // mean | invstd | sc | sh
+  pdl_wait();
   const int N = node_off_v[B];
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
   using TC = TileCols<H>;
@@ -249,6 +256,7 @@ gin_bn_tail_kernel(int mode, const int32_t* __restrict__ node_off_v, int B,
   __shared__ float coef_a[4 * H];
   __shared__ float coef_b[4 * H];
   __shared__ float red[2 * 1024];
+  pdl_wait();
   const int N = node_off_v[B];
   const int tid = threadIdx.x;
   // BN_a running stats are updated by mode 0 only, BN_b's by mode 1 only (once each)
@@ -342,6 +350,7 @@ gin_pool_kernel(int L, const int32_t* __restrict__ node_off_v, int B, const int3
                 double* __restrict__ pool_acc, const float* __restrict__ z2_last, BnTailArgs tail) {
   __shared__ int gid[GCCB_TILE_ROWS];
   __shared__ float coef_a[4 * H], coef_b[4 * H];
+  pdl_wait();
   const int N = node_off_v[B];
   const int tid = threadIdx.x;
   if (z2_last) bn_tail_prepare(tail, N, H, coef_a, coef_b);
@@ -454,6 +463,7 @@ gin_pool_predict_kernel(GinDims d, const int32_t* __restrict__ node_off_v, int B
   __shared__ float score[G][H];
   const int g0 = blockIdx.x * G, tid = threadIdx.x;
   const int ng = min(G, B - g0);
+  pdl_wait();
   if (node_off_v[B] < 0) {                               // view published empty: defined (zero) outputs, the
     for (int i = tid; i < ng * H; i += 256) {            // optimiser / enqueue skip the step (gccb200.h)
       score_out[(size_t)g0 * H + i] = 0.f;
@@ -576,11 +586,12 @@ static int run_forward(const FwdArgs& a) {
   const int tiles = (cap + GCCB_TILE_ROWS - 1) / GCCB_TILE_ROWS;
   const int grid = tiles < 4 * GCCB_NUM_SMS ? tiles : 4 * GCCB_NUM_SMS;   // 4 waves at most
   const int use_running = a.bn_train ? 0 : 1, upd = a.bn_train ? 1 : 0;
-  // BatchNorm statistics and the pooling accumulators are adjacent: one memset
-  cudaMemsetAsync(stats, 0, a.al.pool_acc + (size_t)d.L * B * a.al.PW * sizeof(double) - a.al.stats,
-                  (cudaStream_t)a.stream);
-  GCCB_LAUNCH(gin_build_x0_kernel, grid, 256, 0, a.stream, d, node_off_v, B, pos_v, sub_deg, graph_id,
-              a.params + a.lay.emb, x0);
+  // Every kernel of the SIMT forward is a programmatic dependent of the one before it (common.cuh).  The BatchNorm
+  // statistics and the pooling accumulators are adjacent; gin_build_x0_kernel zeroes them, so that no memset node
+  // breaks the chain.
+  const int64_t n_zero = (int64_t)((a.al.pool_acc + (size_t)d.L * B * a.al.PW * sizeof(double) - a.al.stats) / sizeof(double));
+  GCCB_LAUNCH_PDL(gin_build_x0_kernel, grid, 256, 0, a.stream, d, node_off_v, B, pos_v, sub_deg, graph_id,
+                  a.params + a.lay.emb, x0, stats, n_zero);
   const float* hin = x0;
   BnTailArgs below{};                 // BatchNorm tail of layer l-1, applied by the kernel that reads its output
   for (int l = 0; l < d.L - 1; ++l) {
@@ -599,27 +610,27 @@ static int run_forward(const FwdArgs& a) {
       auto k = gin_agg_gemm1_kernel<GCCB_DINP, H, false>;
       size_t sm = smem_gemm<GCCB_DINP, H>();
       gccb::ensure_dyn_smem(k, sm);
-      GCCB_LAUNCH(k, grid, 256, sm, a.stream, node_off_v, B, indptr, indices, hin, P + a.lay.w1[l], d.din,
-                  P + a.lay.b1[l], 0.0f, a_l, z1, s1, BnTailArgs{});
+      GCCB_LAUNCH_PDL(k, grid, 256, sm, a.stream, node_off_v, B, indptr, indices, hin, P + a.lay.w1[l], d.din,
+                      P + a.lay.b1[l], 0.0f, a_l, z1, s1, BnTailArgs{});
     } else {
       // hin = z2 of layer l-1; its BatchNorm tail (below) is applied on the gather, h[l-1] written on the way
       auto k = gin_agg_gemm1_kernel<H, H, true>;
       size_t sm = smem_gemm<H, H>() + 4 * H * sizeof(float);
       gccb::ensure_dyn_smem(k, sm);
-      GCCB_LAUNCH(k, grid, 256, sm, a.stream, node_off_v, B, indptr, indices, hin, P + a.lay.w1[l], H,
-                  P + a.lay.b1[l], 0.0f, a_l, z1, s1, below);
+      GCCB_LAUNCH_PDL(k, grid, 256, sm, a.stream, node_off_v, B, indptr, indices, hin, P + a.lay.w1[l], H,
+                      P + a.lay.b1[l], 0.0f, a_l, z1, s1, below);
     }
     {
       auto k = gin_bn_gemm2_kernel<H>;
       size_t sm = smem_gemm<H, H>();
       gccb::ensure_dyn_smem(k, sm);
-      GCCB_LAUNCH(k, grid, 256, sm, a.stream, node_off_v, B, z1, s1, P + a.lay.bn1_w[l], P + a.lay.bn1_b[l],
-                  d.bn_eps, run1, use_running, upd, d.bn_mom, P + a.lay.w2[l], P + a.lay.b2[l], z2, sa);
+      GCCB_LAUNCH_PDL(k, grid, 256, sm, a.stream, node_off_v, B, z1, s1, P + a.lay.bn1_w[l], P + a.lay.bn1_b[l],
+                      d.bn_eps, run1, use_running, upd, d.bn_mom, P + a.lay.w2[l], P + a.lay.b2[l], z2, sa);
     }
     auto kt = gin_bn_tail_kernel<H>;
-    GCCB_LAUNCH(kt, grid, 256, 0, a.stream, 0, node_off_v, B, z2, sa, P + a.lay.bna_w[l], P + a.lay.bna_b[l],
-                runa, sb, P + a.lay.bnb_w[l], P + a.lay.bnb_b[l], runb, d.bn_eps, use_running, upd,
-                d.bn_mom, sb, hout);
+    GCCB_LAUNCH_PDL(kt, grid, 256, 0, a.stream, 0, node_off_v, B, z2, sa, P + a.lay.bna_w[l], P + a.lay.bna_b[l],
+                    runa, sb, P + a.lay.bnb_w[l], P + a.lay.bnb_b[l], runb, d.bn_eps, use_running, upd,
+                    d.bn_mom, sb, hout);
     below = BnTailArgs{sa, P + a.lay.bna_w[l], P + a.lay.bna_b[l], runa, sb, P + a.lay.bnb_w[l], P + a.lay.bnb_b[l],
                        runb, d.bn_eps, d.bn_mom, use_running, upd, hout};
     hin = z2;
@@ -627,12 +638,12 @@ static int run_forward(const FwdArgs& a) {
   const uint32_t keep = (uint32_t)fmin((1.0 - (double)d.drop_p) * 4294967296.0, 4294967295.0);
   double* pool_acc = (double*)(a.acts + a.al.pool_acc);
   auto kpl = gin_pool_kernel<H>;
-  GCCB_LAUNCH(kpl, grid, 256, 0, a.stream, d.L, node_off_v, B, graph_id, (const float*)x0, a.d_hptrs, a.al.PW,
-              pool_acc, hin, below);
+  GCCB_LAUNCH_PDL(kpl, grid, 256, 0, a.stream, d.L, node_off_v, B, graph_id, (const float*)x0, a.d_hptrs, a.al.PW,
+                  pool_acc, hin, below);
   auto kp = gin_pool_predict_kernel<H>;
-  GCCB_LAUNCH(kp, (B + GCCB_GPB - 1) / GCCB_GPB, 256, 0, a.stream, d, node_off_v, B, (const double*)pool_acc, a.params, a.d_offs, a.d_offs + 8,
-              a.al.PW, a.drop_key, a.drop_step, a.drop_base, keep, (float*)(a.acts + a.al.pooled),
-              (float*)(a.acts + a.al.score), a.feat, a.pooled_user);
+  GCCB_LAUNCH_PDL(kp, (B + GCCB_GPB - 1) / GCCB_GPB, 256, 0, a.stream, d, node_off_v, B, (const double*)pool_acc, a.params,
+                  a.d_offs, a.d_offs + 8, a.al.PW, a.drop_key, a.drop_step, a.drop_base, keep,
+                  (float*)(a.acts + a.al.pooled), (float*)(a.acts + a.al.score), a.feat, a.pooled_user);
   return check_launch("gccb_gin_forward");
 }
 
@@ -792,7 +803,7 @@ static int run_forward_tc(const FwdArgs& a) {
   const int use_running = a.bn_train ? 0 : 1, upd = a.bn_train ? 1 : 0;
   cudaMemsetAsync(stats, 0, a.al.pool_acc + (size_t)d.L * B * a.al.PW * sizeof(double) - a.al.stats, st);
   GCCB_LAUNCH(gin_build_x0_kernel, grid, 256, 0, a.stream, d, node_off_v, B, pos_v, sub_deg, graph_id,
-              a.params + a.lay.emb, x0);
+              a.params + a.lay.emb, x0, (double*)nullptr, (int64_t)0);
   {
     dim3 gw(64, d.L - 1);
     GCCB_LAUNCH(gin_cast_weights_kernel, gw, 256, 0, a.stream, d, a.lay, a.params, a.acts, a.al);
@@ -878,6 +889,7 @@ namespace gccb {
 __global__ void gin_fill_tables_kernel(char* acts, ActsLayout al, gccb_gin_layout_t lay, int L,
                                        const float** hptrs, int64_t* offs, int64_t* nbt,
                                        const int32_t* n_valid) {
+  pdl_wait();
   int t = threadIdx.x;
   if (t < L - 1) hptrs[t] = (const float*)(acts + al.h[t]);
   if (t < 8) { offs[t] = lay.wp[t]; offs[8 + t] = lay.bp[t]; }
@@ -912,9 +924,9 @@ extern "C" int gccb_gin_forward(const gccb_gin_cfg_t* cfg, const gccb_batch_t* b
   char* tail = (char*)acts + a.al.total;
   a.d_hptrs = (const float**)tail;
   a.d_offs = (int64_t*)(tail + 8 * sizeof(void*));
-  GCCB_LAUNCH(gin_fill_tables_kernel, 1, 32, 0, stream, (char*)acts, a.al, a.lay, a.d.L, a.d_hptrs, a.d_offs,
-              bn_train ? num_batches_tracked : (int64_t*)nullptr,
-              (const int32_t*)(batch->node_off + (size_t)view * (batch->batch + 1) + batch->batch));
+  GCCB_LAUNCH_PDL(gin_fill_tables_kernel, 1, 32, 0, stream, (char*)acts, a.al, a.lay, a.d.L, a.d_hptrs, a.d_offs,
+                  bn_train ? num_batches_tracked : (int64_t*)nullptr,
+                  (const int32_t*)(batch->node_off + (size_t)view * (batch->batch + 1) + batch->batch));
 #ifndef GCCB_EMU
   if (a.d.tc) return a.d.H == 128 ? run_forward_tc<128>(a) : run_forward_tc<256>(a);
 #endif

@@ -126,13 +126,15 @@ nce_loss_kernel(const float* __restrict__ out, int B, int C, int label_mode,
 template <int KPT, int DU>
 __global__ void __launch_bounds__(256)
 infonce_partial_tiled_kernel(const float* __restrict__ q, const float* __restrict__ mem, int B, int K,
-                             float invT, float* __restrict__ part) {
+                             float invT, float* __restrict__ part, float* __restrict__ stats) {
   constexpr int CK = 32 * KPT, d = 32 * DU, RB = GCCB_NCE_RB2;
   GCCB_DYN_SMEM(float, smem);
   float* qs = smem;
   float* ms = qs + RB * d;
   float* ps = ms + (size_t)CK * (d + 1);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  pdl_wait();
+  if (blockIdx.x == 0 && blockIdx.y == 0 && tid < 2) stats[tid] = 0.f;   // infonce_merge_kernel accumulates them
   const int i0 = blockIdx.y * RB, j0 = blockIdx.x * CK;
   const int nk = min(CK, K - j0);
   for (int idx = tid; idx < RB * d; idx += 256) {
@@ -222,6 +224,7 @@ infonce_merge_kernel(const float* __restrict__ q, const float* __restrict__ k,
   __shared__ float red_s[4];
   __shared__ float bc[3];
   const int i = blockIdx.x, tid = threadIdx.x;
+  pdl_wait();
   float s = 0.f;
   for (int c = tid; c < d; c += 128) s = fmaf(q[(size_t)i * d + c], k[(size_t)i * d + c], s);
   s = warp_sum(s);
@@ -258,6 +261,7 @@ infonce_merge_kernel(const float* __restrict__ q, const float* __restrict__ k,
 __global__ void moco_enqueue_kernel(float* __restrict__ mem, const float* __restrict__ k, int B, int d,
                                     int K, const int64_t* __restrict__ index_dev, int parts, int64_t part_stride,
                                     const int32_t* __restrict__ skip_word, int32_t skip_mask) {
+  pdl_wait();
   if (skip_word && (*skip_word & skip_mask)) return;   // step skipped (empty view): the queue keeps its keys
   const int64_t base = *index_dev;
   const int per = B * d, total = parts * per;
@@ -270,6 +274,7 @@ __global__ void moco_enqueue_kernel(float* __restrict__ mem, const float* __rest
 }
 __global__ void moco_advance_kernel(int64_t* index_dev, int B, int K, const int32_t* __restrict__ skip_word,
                                     int32_t skip_mask) {
+  pdl_wait();
   if (skip_word && (*skip_word & skip_mask)) return;
   if (threadIdx.x == 0 && blockIdx.x == 0) *index_dev = (*index_dev + B) % K;
 }
@@ -535,25 +540,29 @@ extern "C" int gccb_infonce_fused(const float* q, const float* k, const float* m
   }
   const int ck = infonce_ck(d);
   const int nch = (K + ck - 1) / ck;
-  cudaMemsetAsync(stats, 0, 2 * sizeof(float), (cudaStream_t)stream);
 #ifndef GCCB_EMU
-  if (nce_use_tc(B, d, K)) return infonce_tc(q, k, memory, B, d, K, T, stats, dq, (char*)workspace, (cudaStream_t)stream);
+  if (nce_use_tc(B, d, K)) {
+    cudaMemsetAsync(stats, 0, 2 * sizeof(float), (cudaStream_t)stream);
+    return infonce_tc(q, k, memory, B, d, K, T, stats, dq, (char*)workspace, (cudaStream_t)stream);
+  }
 #endif
+  // both kernels are programmatic dependents of the kernel before them (common.cuh); the partial pass zeroes the
+  // statistics the merge accumulates, so that no memset node breaks the chain
   const size_t smem = ((size_t)GCCB_NCE_RB2 * d + (size_t)ck * (d + 1) + (size_t)GCCB_NCE_RB2 * ck) * 4;
   dim3 grid(nch, (B + GCCB_NCE_RB2 - 1) / GCCB_NCE_RB2);
 #define GCCB_NCE_TILED(KPT, DU)                                                              \
   do {                                                                                       \
     auto kt = infonce_partial_tiled_kernel<KPT, DU>;                                         \
     gccb::ensure_dyn_smem(kt, smem);                                                         \
-    GCCB_LAUNCH(kt, grid, 256, smem, stream, q, memory, B, K, 1.0f / T, (float*)workspace); \
+    GCCB_LAUNCH_PDL(kt, grid, 256, smem, stream, q, memory, B, K, 1.0f / T, (float*)workspace, stats); \
   } while (0)
   if (d == 32) GCCB_NCE_TILED(4, 1);
   else if (d == 64) GCCB_NCE_TILED(4, 2);
   else if (d == 128) GCCB_NCE_TILED(4, 4);
   else GCCB_NCE_TILED(2, 8);
 #undef GCCB_NCE_TILED
-  GCCB_LAUNCH(infonce_merge_kernel, B, 128, 0, stream, q, k, (const float*)workspace, B, d, nch, 1.0f / T,
-              stats, dq);
+  GCCB_LAUNCH_PDL(infonce_merge_kernel, B, 128, 0, stream, q, k, (const float*)workspace, B, d, nch, 1.0f / T,
+                  stats, dq);
   return check_launch("gccb_infonce_fused");
 }
 
@@ -566,9 +575,9 @@ extern "C" int gccb_moco_enqueue(float* memory, const float* k, int32_t B, int32
   }
   int blocks = (parts * B * d + 255) / 256;
   if (blocks > 1184) blocks = 1184;
-  GCCB_LAUNCH(moco_enqueue_kernel, blocks, 256, 0, stream, memory, k, B, d, K, (const int64_t*)index_dev, parts,
-              part_stride, skip_word, skip_mask);
-  GCCB_LAUNCH(moco_advance_kernel, 1, 32, 0, stream, index_dev, parts * B, K, skip_word, skip_mask);
+  GCCB_LAUNCH_PDL(moco_enqueue_kernel, blocks, 256, 0, stream, memory, k, B, d, K, (const int64_t*)index_dev, parts,
+                  part_stride, skip_word, skip_mask);
+  GCCB_LAUNCH_PDL(moco_advance_kernel, 1, 32, 0, stream, index_dev, parts * B, K, skip_word, skip_mask);
   return check_launch("gccb_moco_enqueue");
 }
 

@@ -13,6 +13,7 @@ namespace gccb {
 __global__ void __launch_bounds__(256)
 gradnorm_kernel(const float* __restrict__ g, int64_t n, float scale, double* __restrict__ acc) {
   __shared__ double red_s[8];
+  pdl_wait();
   double s = 0.0;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     double v = (double)g[i] * (double)scale;
@@ -39,6 +40,7 @@ clip_update_ema_kernel(float* __restrict__ p, const float* __restrict__ g, float
                        const int32_t* __restrict__ skip_word, int32_t skip_mask) {
   // a batch whose view was published empty (capacity overflow) must not move the weights: the whole
   // update (optimiser state, parameters, momentum encoder) is a no-op for that step
+  pdl_wait();
   if (skip_word && (*skip_word & skip_mask)) return;
   const float total = (float)sqrt(*sumsq);
   float coef = 1.0f;
@@ -81,7 +83,9 @@ using namespace gccb;
 namespace {
 
 // The clip norm (gradnorm_kernel) then the update of every live entry and the EMA of all n_all entries
-// (clip_update_ema_kernel<Rule>), on `stream`.
+// (clip_update_ema_kernel<Rule>), on `stream`, both programmatic dependents of the kernel before them
+// (common.cuh).  The norm's accumulator stays a memset: every block of gradnorm_kernel adds to it, so no block of
+// it could zero it first, and the call has no earlier kernel.
 template <class Rule>
 int clip_update_ema(const char* name, float* p, const float* g, float* s0, float* s1, float* p_ema, int64_t n_live,
                     int64_t n_all, const float* hyper, Rule rule, float weight_decay, float clip_norm, float alpha,
@@ -90,12 +94,12 @@ int clip_update_ema(const char* name, float* p, const float* g, float* s0, float
   cudaMemsetAsync(workspace, 0, sizeof(double), (cudaStream_t)stream);
   int blocks = (int)((n_live + 255) / 256);
   if (blocks > 4 * GCCB_NUM_SMS) blocks = 4 * GCCB_NUM_SMS;
-  GCCB_LAUNCH(gradnorm_kernel, blocks, 256, 0, stream, g, n_live, grad_scale, workspace);
+  GCCB_LAUNCH_PDL(gradnorm_kernel, blocks, 256, 0, stream, g, n_live, grad_scale, workspace);
   int blocks2 = (int)((n_all + 255) / 256);
   if (blocks2 > 1184) blocks2 = 1184;
-  GCCB_LAUNCH(clip_update_ema_kernel<Rule>, blocks2, 256, 0, stream, p, g, s0, s1, p_ema, n_live, n_all, hyper,
-              rule, weight_decay, clip_norm, alpha, grad_scale, (const double*)workspace, grad_norm_out, skip_word,
-              skip_mask);
+  GCCB_LAUNCH_PDL(clip_update_ema_kernel<Rule>, blocks2, 256, 0, stream, p, g, s0, s1, p_ema, n_live, n_all, hyper,
+                  rule, weight_decay, clip_norm, alpha, grad_scale, (const double*)workspace, grad_norm_out, skip_word,
+                  skip_mask);
   return check_launch(name);
 }
 
