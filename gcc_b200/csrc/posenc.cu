@@ -143,10 +143,16 @@ posenc_classify_kernel(const int64_t* __restrict__ counters, const int32_t* __re
   if (tid < GCCB_EIG_NCLASS) counts[tid] = base[tid];
 }
 
-// Two-sided Jacobi specialised for the even-order Ritz problem (m = 48): per round ONE thread per pair
-// derives (c, s); then every thread applies BOTH sides of the similarity transform to whole 2 x 2
-// blocks (rows of pair a, columns of pair b) -- no barrier between the row and the column update --
-// and rotates V.  Two barriers per round instead of three, independent items unrolled for ILP.
+// Two-sided Jacobi specialised for the even-order Ritz problem (m = 48): per round ONE lane of warp 0 per
+// pair derives (c, s); then every thread applies BOTH sides of the similarity transform to whole 2 x 2
+// blocks (rows of pair a, columns of pair b) -- no barrier between the row and the column update.
+// Only A is on the round-to-round critical path, so two things stay off it:
+//  - rounds that rotate nothing leave A unchanged: warp 0 steps over them on its own (warp votes only)
+//    and publishes the next round that rotates, so an idle round costs no CTA barrier;
+//  - V <- V J of a round is applied by warps 1.. while warp 0 derives the next round's rotations (the
+//    columns of V are not read by the rotation test), not between the A update and its barrier.
+// Each element goes through the same rotations in the same order as with one update per round, so the
+// result does not depend on this schedule.
 // `tol`: relative skip threshold (adaptive: the Ritz vectors need no more accuracy than the
 // current outer residual).
 template <int NT>
@@ -154,13 +160,13 @@ __device__ __forceinline__ int jacobi_ritz48(float* A, float* V, float* cs /*[64
                                               float tol, int max_sweeps, long long* n_work = nullptr,
                                               long long* n_idle = nullptr) {
   constexpr int M = GCCB_CF_B, HALF = M / 2;
+  static_assert(NT >= 64, "V is rotated by the warps after the first");
   const int tid = threadIdx.x;
-  // One 16-byte record per pair and round: (p | q << 16, c, s, -), written in COMPACTED order: slots
-  // [0, nr) hold the pairs that rotate this round, the others fill the array from the top.  A block / column
-  // update then costs one 128-bit shared-memory load per pair instead of five scalar ones (the rounds are
-  // bound by shared-memory instruction throughput: three CTAs share an SM).  Two copies alternate between
-  // rounds, so an idle round (nr == 0) costs ONE barrier: the next round's writer never touches the copy a
-  // slow reader may still be looking at.  (cs / pq of the caller are no longer used.)
+  // One 16-byte record per pair of a rotating round: (p | q << 16, c, s, -), written in COMPACTED order:
+  // slots [0, nr) hold the pairs that rotate, the others fill the array from the top.  A block / column
+  // update then costs one 128-bit shared-memory load per pair instead of five scalar ones.  Two copies
+  // alternate between published rounds: warp 0 writes one while warps 1.. still rotate V with the other.
+  // (cs / pq of the caller are no longer used.)
   __shared__ float4 rec2[2][HALF];
   __shared__ int nrot2[2];
   (void)cs; (void)pq;
@@ -169,7 +175,10 @@ __device__ __forceinline__ int jacobi_ritz48(float* A, float* V, float* cs /*[64
     V[j * LD + i] = i == j ? 1.0f : 0.f;
   }
   __syncthreads();
-  int sweep = 0;
+  // V <- V J owed for the last published round: warps 1.. apply it while warp 0 looks for the next one.  A sweep
+  // ends with a look that finds no rotating round, so nothing is owed when it ends.
+  int pend_nr = 0, pend_buf = 0;
+  int sweep = 0, buf = 0;
   for (; sweep < max_sweeps; ++sweep) {
     // One look at the whole triangle decides whether another sweep is needed (the same test the rounds
     // apply): a converged matrix costs one barrier instead of M - 1 idle rounds.
@@ -181,43 +190,62 @@ __device__ __forceinline__ int jacobi_ritz48(float* A, float* V, float* cs /*[64
       }
       if (!__syncthreads_or(any)) break;
     }
-    for (int r = 0; r < M - 1; ++r) {
-      float4* rec = rec2[r & 1];
-      if (tid < 32) {                                      // warp 0: one lane per pair
-        bool rot = false;
-        int p = 0, q = 0;
-        float c = 1.0f, sn = 0.f;
-        if (tid < HALF) {
-          if (tid == 0) { p = M - 1; q = r; }
-          else { p = (r + tid) % (M - 1); q = (r + M - 1 - tid) % (M - 1); }
-          if (p > q) { int t = p; p = q; q = t; }
-          const float app = A[p * LD + p], aqq = A[q * LD + q], apq = A[q * LD + p];
-          // (diagonal of G = H + 2I lies in [1, 3]: the arithmetic mean is as good a scale as the geometric one)
-          if (fabsf(apq) > tol * 0.5f * (fabsf(app) + fabsf(aqq))) {
-            // t = sgn(zeta) / (|zeta| + sqrt(1 + zeta^2)), zeta = d / (2 apq), without dividing by apq;
-            // fast division / reciprocal square root: this dependent chain is on the critical path of
-            // every round, and a 2-ulp rotation error is far below the Ritz tolerance
-            const float d = aqq - app;
-            const float two_apq = 2.0f * apq;
-            const float den = fabsf(d) + __fsqrt_rn(fmaf(d, d, two_apq * two_apq));
-            const float t = __fdividef(d >= 0.f ? two_apq : -two_apq, den);
-            c = rsqrtf(fmaf(t, t, 1.0f));
-            sn = c * t;
-            rot = true;
+    int r = 0;                                           // warp 0's round; the other warps never read it
+    for (;;) {
+      if (tid < 32) {                                    // warp 0: one lane per pair, up to the next rotating round
+        for (; r < M - 1; ++r) {
+          bool rot = false;
+          int p = 0, q = 0;
+          float c = 1.0f, sn = 0.f;
+          if (tid < HALF) {
+            if (tid == 0) { p = M - 1; q = r; }
+            else { p = (r + tid) % (M - 1); q = (r + M - 1 - tid) % (M - 1); }
+            if (p > q) { int t = p; p = q; q = t; }
+            const float app = A[p * LD + p], aqq = A[q * LD + q], apq = A[q * LD + p];
+            // (diagonal of G = H + 2I lies in [1, 3]: the arithmetic mean is as good a scale as the geometric one)
+            if (fabsf(apq) > tol * 0.5f * (fabsf(app) + fabsf(aqq))) {
+              // t = sgn(zeta) / (|zeta| + sqrt(1 + zeta^2)), zeta = d / (2 apq), without dividing by apq;
+              // fast division / reciprocal square root: this dependent chain is on the critical path of
+              // every round, and a 2-ulp rotation error is far below the Ritz tolerance
+              const float d = aqq - app;
+              const float two_apq = 2.0f * apq;
+              const float den = fabsf(d) + __fsqrt_rn(fmaf(d, d, two_apq * two_apq));
+              const float t = __fdividef(d >= 0.f ? two_apq : -two_apq, den);
+              c = rsqrtf(fmaf(t, t, 1.0f));
+              sn = c * t;
+              rot = true;
+            }
           }
+          const unsigned mask = __ballot_sync(0xffffffffu, rot);
+          if (mask == 0u) { if (tid == 0 && n_idle) ++*n_idle; continue; }
+          if (tid < HALF) {
+            const int below = __popc(mask & ((1u << tid) - 1u));
+            const int slot = rot ? below : HALF - 1 - (tid - below);
+            rec2[buf][slot] = make_float4(__int_as_float(p | (q << 16)), c, sn, 0.f);
+          }
+          if (tid == 0) nrot2[buf] = __popc(mask);
+          break;
         }
-        const unsigned mask = __ballot_sync(0xffffffffu, rot);
-        if (tid < HALF) {
-          const int below = __popc(mask & ((1u << tid) - 1u));
-          const int slot = rot ? below : HALF - 1 - (tid - below);
-          rec[slot] = make_float4(__int_as_float(p | (q << 16)), c, sn, 0.f);
+        if (r == M - 1 && tid == 0) nrot2[buf] = 0;      // the rest of the sweep rotates nothing
+        ++r;
+      } else {                                           // warps 1..: V <- V J of the last published round
+        const float4* rec = rec2[pend_buf];
+        for (int item = tid - 32; item < pend_nr * M; item += NT - 32) {
+          const int ir = item / M, i = item - ir * M;
+          const float4 rr = rec[ir];
+          const int code = __float_as_int(rr.x);
+          const int p = code & 0xffff, q = code >> 16;
+          const float x = V[p * LD + i], y = V[q * LD + i];
+          V[p * LD + i] = rr.y * x - rr.z * y;
+          V[q * LD + i] = rr.z * x + rr.y * y;
         }
-        if (tid == 0) nrot2[r & 1] = __popc(mask);
       }
       __syncthreads();
-      const int nr = nrot2[r & 1];
-      if (nr == 0) { if (n_idle) ++*n_idle; continue; }
-      if (n_work) ++*n_work;
+      const int nr = nrot2[buf];
+      pend_nr = 0;
+      if (nr == 0) break;
+      if (tid == 0 && n_work) ++*n_work;
+      const float4* rec = rec2[buf];
       // A <- J^T A J on 2x2 blocks (rows of pair a, columns of pair b).  A is symmetric and only its canonical
       // triangle T(x, y) = A[max(x, y) * LD + min(x, y)] is kept up to date (the rotation test above and the
       // caller read nothing else), so each UNORDERED pair of slots {a, b} is one work item instead of two;
@@ -257,17 +285,8 @@ __device__ __forceinline__ int jacobi_ritz48(float* A, float* V, float* cs /*[64
         A[i_c] = s1 * a2 + c1 * c3;
         A[i_d] = s1 * b2 + c1 * d2;
       }
-      // V <- V J: only the columns of rotating pairs
-      for (int item = tid; item < nr * M; item += NT) {
-        const int ir = item / M, i = item - ir * M;
-        const float4 rr = rec[ir];
-        const int code = __float_as_int(rr.x);
-        const int p = code & 0xffff, q = code >> 16;
-        const float x = V[p * LD + i], y = V[q * LD + i];
-        V[p * LD + i] = rr.y * x - rr.z * y;
-        V[q * LD + i] = rr.z * x + rr.y * y;
-      }
       __syncthreads();
+      pend_nr = nr; pend_buf = buf; buf ^= 1;
     }
   }
   return sweep;
@@ -318,45 +337,45 @@ struct SubCsr {
 };
 
 // dst[r][c] = alpha * (sum_{j in N(r)} w_rj src[j][c] - cen * src[r][c]) - beta * dst[r][c]
-// (beta == 0: dst is write-only).  One warp per row; lane owns columns lane and 32 + lane.
+// (beta == 0: dst is write-only).  One half-warp per row, two rows per warp at a time: lane l of a half owns
+// columns l, 16 + l and 32 + l, so every lane works (a warp per row left 16 of its 64 column slots empty) and
+// the dependent index -> neighbour-row loads of two rows are in flight together.  Each column's sum runs in
+// the same order whatever the row-to-lane assignment.  The epilogue's fused multiply-adds are written out: left
+// to the compiler, alpha * t - beta * d may be fused either way, and the rounding would depend on the code around it.
 __device__ __forceinline__ void spmm_cheb(const SubCsr& S, const float* __restrict__ src, float* __restrict__ dst,
                                           int ld, float alpha, float cen, float beta) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  const bool hi = lane < GCCB_CF_B - 32;
-  for (int r = warp; r < S.n; r += nw) {
+  static_assert(GCCB_CF_B == 48, "three 16-column strips per row");
+  const int lane = threadIdx.x & 15, half = (threadIdx.x >> 4) & 1;
+  const int warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  for (int r = 2 * warp + half; r < S.n; r += 2 * nw) {
     const int beg = S.indptr[S.noff + r], end = S.indptr[S.noff + r + 1];
     const float dr = S.dinv[r];
-    float a0 = 0.f, a1 = 0.f, b0 = 0.f, b1 = 0.f;
+    float a[3] = {0.f, 0.f, 0.f}, b[3] = {0.f, 0.f, 0.f};
     int e = beg;
     for (; e + 3 < end; e += 4) {                         // four edges (gathers) in flight
       const int j0 = S.indices[e] - S.noff, j1 = S.indices[e + 1] - S.noff;
       const int j2 = S.indices[e + 2] - S.noff, j3 = S.indices[e + 3] - S.noff;
-      const float x0 = src[(size_t)j0 * ld + lane], x1 = src[(size_t)j1 * ld + lane];
-      const float x2 = src[(size_t)j2 * ld + lane], x3 = src[(size_t)j3 * ld + lane];
-      float y0 = 0.f, y1 = 0.f, y2 = 0.f, y3 = 0.f;
-      if (hi) {
-        y0 = src[(size_t)j0 * ld + 32 + lane]; y1 = src[(size_t)j1 * ld + 32 + lane];
-        y2 = src[(size_t)j2 * ld + 32 + lane]; y3 = src[(size_t)j3 * ld + 32 + lane];
-      }
       const float w0 = dr * S.dinv[j0], w1 = dr * S.dinv[j1], w2 = dr * S.dinv[j2], w3 = dr * S.dinv[j3];
-      a0 = fmaf(w0, x0, a0); b0 = fmaf(w1, x1, b0); a0 = fmaf(w2, x2, a0); b0 = fmaf(w3, x3, b0);
-      a1 = fmaf(w0, y0, a1); b1 = fmaf(w1, y1, b1); a1 = fmaf(w2, y2, a1); b1 = fmaf(w3, y3, b1);
+#pragma unroll
+      for (int s = 0; s < 3; ++s) {
+        const int c = 16 * s + lane;
+        const float x0 = src[(size_t)j0 * ld + c], x1 = src[(size_t)j1 * ld + c];
+        const float x2 = src[(size_t)j2 * ld + c], x3 = src[(size_t)j3 * ld + c];
+        a[s] = fmaf(w0, x0, a[s]); b[s] = fmaf(w1, x1, b[s]); a[s] = fmaf(w2, x2, a[s]); b[s] = fmaf(w3, x3, b[s]);
+      }
     }
     for (; e < end; ++e) {
       const int j0 = S.indices[e] - S.noff;
       const float w0 = dr * S.dinv[j0];
-      a0 = fmaf(w0, src[(size_t)j0 * ld + lane], a0);
-      if (hi) a1 = fmaf(w0, src[(size_t)j0 * ld + 32 + lane], a1);
+#pragma unroll
+      for (int s = 0; s < 3; ++s) a[s] = fmaf(w0, src[(size_t)j0 * ld + 16 * s + lane], a[s]);
     }
-    a0 += b0; a1 += b1;
-    const size_t o = (size_t)r * ld + lane;
-    float v = alpha * (a0 - cen * src[o]);
-    if (beta != 0.f) v -= beta * dst[o];
-    dst[o] = v;
-    if (hi) {
-      float v1 = alpha * (a1 - cen * src[o + 32]);
-      if (beta != 0.f) v1 -= beta * dst[o + 32];
-      dst[o + 32] = v1;
+#pragma unroll
+    for (int s = 0; s < 3; ++s) {
+      const size_t o = (size_t)r * ld + 16 * s + lane;
+      float v = alpha * fmaf(-cen, src[o], a[s] + b[s]);
+      if (beta != 0.f) v = fmaf(-beta, dst[o], v);
+      dst[o] = v;
     }
   }
 }
@@ -422,7 +441,11 @@ __device__ __forceinline__ void posenc_chfsi_item(const int item, const int32_t*
   __shared__ int perm[CB];
   __shared__ float s_bc[2];
   __shared__ float sgn[32];
-  __shared__ float rd4[GCCB_GS_PANEL * CB];      // panel Gram-Schmidt: dots of the 4 panel columns with all columns
+  // panel Gram-Schmidt: dots of the 4 panel columns with all columns, column-major (rd4[c * 4 + q] = y_q . x_c), so
+  // the update pass reads the four coefficients of a column with one 128-bit broadcast load
+  static_assert(GCCB_GS_PANEL == 4, "one float4 of panel dots per column");
+  __shared__ float4 rd4v[CB];
+  float* rd4 = reinterpret_cast<float*>(rd4v);
   __shared__ float pl[16];                        // inverse of the panel's 4 x 4 Cholesky factor (lower triangle)
   __shared__ int pflag;
   float* Ws = WT;
@@ -584,7 +607,7 @@ __device__ __forceinline__ void posenc_chfsi_item(const int item, const int32_t*
             float sacc = 0.f;
 #pragma unroll
             for (int w = 0; w < nwu; ++w) sacc += part[(w * GCCB_GS_PANEL + q) * CB + c];
-            rd4[t] = sacc;
+            rd4[c * GCCB_GS_PANEL + q] = sacc;
           }
           __syncthreads();
         }
@@ -595,15 +618,16 @@ __device__ __forceinline__ void posenc_chfsi_item(const int item, const int32_t*
           float gp = 0.f;
           if (lane < 10) {
             float sacc = 0.f;
-            for (int i = 0; i < j0; ++i) sacc = fmaf(rd4[a * CB + i], rd4[b * CB + i], sacc);
-            gp = rd4[a * CB + j0 + b] - sacc;
+            for (int i = 0; i < j0; ++i) sacc = fmaf(rd4[i * GCCB_GS_PANEL + a], rd4[i * GCCB_GS_PANEL + b], sacc);
+            gp = rd4[(j0 + b) * GCCB_GS_PANEL + a] - sacc;
           }
           float g[10];
 #pragma unroll
           for (int q = 0; q < 10; ++q) g[q] = __shfl_sync(0xffffffffu, gp, q);
           if (lane == 0) {
             // g: 0 (0,0) | 1 (1,0) 2 (1,1) | 3 (2,0) 4 (2,1) 5 (2,2) | 6 (3,0) 7 (3,1) 8 (3,2) 9 (3,3)
-            const float yy0 = rd4[0 * CB + j0], yy1 = rd4[1 * CB + j0 + 1], yy2 = rd4[2 * CB + j0 + 2], yy3 = rd4[3 * CB + j0 + 3];
+            const float yy0 = rd4[j0 * GCCB_GS_PANEL], yy1 = rd4[(j0 + 1) * GCCB_GS_PANEL + 1];
+            const float yy2 = rd4[(j0 + 2) * GCCB_GS_PANEL + 2], yy3 = rd4[(j0 + 3) * GCCB_GS_PANEL + 3];
             int flag = 0;
             const bool tiny = !(g[0] > 1e-30f) || !(g[2] > 1e-30f) || !(g[5] > 1e-30f) || !(g[9] > 1e-30f);
             const bool again = !(g[0] > 0.5f * yy0) || !(g[2] > 0.5f * yy1) || !(g[5] > 0.5f * yy2) || !(g[9] > 0.5f * yy3);
@@ -648,10 +672,11 @@ __device__ __forceinline__ void posenc_chfsi_item(const int item, const int32_t*
           float v0 = row[j0], v1 = row[j0 + 1], v2 = row[j0 + 2], v3 = row[j0 + 3];
           for (int i = 0; i < j0; ++i) {
             const float q = row[i];
-            v0 = fmaf(-rd4[i], q, v0);
-            v1 = fmaf(-rd4[CB + i], q, v1);
-            v2 = fmaf(-rd4[2 * CB + i], q, v2);
-            v3 = fmaf(-rd4[3 * CB + i], q, v3);
+            const float4 d = rd4v[i];
+            v0 = fmaf(-d.x, q, v0);
+            v1 = fmaf(-d.y, q, v1);
+            v2 = fmaf(-d.z, q, v2);
+            v3 = fmaf(-d.w, q, v3);
           }
           row[j0] = pl[0] * v0;
           row[j0 + 1] = fmaf(pl[1], v0, pl[2] * v1);
@@ -750,26 +775,45 @@ __device__ __forceinline__ void posenc_chfsi_item(const int item, const int32_t*
       perm[rank] = j;                                   // descending: perm[0] = largest
     }
     __syncthreads();
-    // ---- X <- Q W[:, perm]: one warp per row, lanes over output columns, in place -----------------
-    for (int r = warp; r < n; r += NW) {
+    // ---- X <- Q W[:, perm]: one warp per XQW_R rows, lanes over output columns, in place -----------------
+    // (each W element a lane loads serves XQW_R rows: the pass is bound by shared-memory loads)
+    constexpr int XQW_R = 4;
+    for (int r0 = warp; r0 < n; r0 += XQW_R * NW) {
       const float* w0 = Ws + perm[lane] * LD;
       const float* w1 = Ws + perm[hi ? 32 + lane : 0] * LD;
-      const float* row = X + (size_t)r * ld;
-      float a0 = 0.f, a1 = 0.f;
+      const float* row[XQW_R];
+#pragma unroll
+      for (int u = 0; u < XQW_R; ++u) row[u] = X + (size_t)(r0 + u * NW < n ? r0 + u * NW : r0) * ld;   // past n: not stored
+      float a0[XQW_R], a1[XQW_R];
       if (ritz_skipped) {                                // a column permutation
-        a0 = row[perm[lane]];
-        a1 = row[perm[hi ? 32 + lane : 0]];
+#pragma unroll
+        for (int u = 0; u < XQW_R; ++u) {
+          a0[u] = row[u][perm[lane]];
+          a1[u] = row[u][perm[hi ? 32 + lane : 0]];
+        }
       } else {
-#pragma unroll 8
+#pragma unroll
+        for (int u = 0; u < XQW_R; ++u) a0[u] = a1[u] = 0.f;
+#pragma unroll 4
         for (int i = 0; i < CB; ++i) {
-          const float q = row[i];                          // broadcast
-          a0 = fmaf(q, w0[i], a0);
-          a1 = fmaf(q, w1[i], a1);
+          const float wa = w0[i], wb = w1[i];
+#pragma unroll
+          for (int u = 0; u < XQW_R; ++u) {
+            const float q = row[u][i];                     // broadcast
+            a0[u] = fmaf(q, wa, a0[u]);
+            a1[u] = fmaf(q, wb, a1[u]);
+          }
         }
       }
-      __syncwarp();                                      // all lanes have read row r before it is overwritten
-      X[(size_t)r * ld + lane] = a0;
-      if (hi) X[(size_t)r * ld + 32 + lane] = a1;
+      __syncwarp();                                      // all lanes have read the rows before they are overwritten
+#pragma unroll
+      for (int u = 0; u < XQW_R; ++u) {
+        const int r = r0 + u * NW;
+        if (r < n) {
+          X[(size_t)r * ld + lane] = a0[u];
+          if (hi) X[(size_t)r * ld + 32 + lane] = a1[u];
+        }
+      }
     }
     __syncthreads();
     GCCB_TICK(4);
