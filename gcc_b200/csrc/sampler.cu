@@ -95,6 +95,15 @@ __device__ __forceinline__ int adj_count(const int32_t* __restrict__ indices, in
 #define GCCB_HUB_LIST 1024     // hub rows per ego-net handled CTA-wide (further ones fall back to one warp each)
 #endif
 #define GCCB_HIT_STAGE 128     // hits of one row parked in shared memory before their pool slot is known
+// Walk CTAs keep the trace in GCCB_WALK_KEYS ints of dynamic shared memory (128 KiB): a sample whose walk budget
+// + HOPCAP exceeds it is walked and induced by the wide kernels below, from a key array in global memory.
+// (The emulator build lowers it, so that the kernel-logic tests reach the wide path on small graphs.)
+#ifndef GCCB_WALK_KEYS
+#define GCCB_WALK_KEYS 32768
+#endif
+#define GCCB_WALK_BUDGET_MAX (GCCB_WALK_KEYS - (int)GCCB_HOPCAP)
+#define GCCB_WIDE_CTAS 32      // wide walk CTAs in flight, each with its own key array; they claim slots in turn
+#define GCCB_WIDE_KEYS_MAX (1 << 30)   // a wide trace's int32 positions: pow2 >= budget + HOPCAP up to 2^30
 
 // Block-wide ascending bitonic sort of a[0..cnt), padded with INT_MAX to a power of two (the buffer must hold it).
 __device__ void block_sort_pad(int* a, int cnt) {
@@ -229,14 +238,15 @@ __device__ int ns_expand(const int64_t* __restrict__ indptr, const int32_t* __re
 }
 
 // RWR node set of one (sample, view) (reference graph_dataset.py:113-130, data_util.py:221-226): the traces from
-// seed64 until `budget` vertices are recorded, sorted and uniqued in keys[]; writes subv[1..n) = the visited vertices
-// but the seed, ascending, and returns n (the caller writes subv[0] = seed).  *steps = recorded vertices.  s_tstar
-// and s_m are the kernel's shared words (s_m is left 0).
+// seed64 until `budget` vertices are recorded, sorted and uniqued in keys[]; writes rest[0..n-1) = the visited
+// vertices but the seed, ascending, and returns n (the caller puts the seed in front).  rest may be keys itself:
+// the unique pass writes each vertex at or below the position it reads it from.  *steps = recorded vertices.
+// s_tstar and s_m are the kernel's shared words (s_m is left 0).
 __device__ __forceinline__ int rwr_node_set(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices,
                                             int budget, uint32_t restart_thresh, uint64_t key, uint64_t sample,
                                             int view, int64_t seed64, int seed, int* keys, int* scan_scratch,
                                             int* s_tstar, int* s_m, int32_t* __restrict__ flags,
-                                            int32_t* __restrict__ subv, int* steps) {
+                                            int32_t* rest, int* steps) {
   const int tid = threadIdx.x;
   if (tid == 0) *s_tstar = 0x7fffffff;
   __syncthreads();
@@ -313,7 +323,7 @@ __device__ __forceinline__ int rwr_node_set(const int64_t* __restrict__ indptr, 
     }
     int cnt;
     int ex = block_scan_excl(head, scan_scratch, &cnt);
-    if (head) subv[1 + n_rest + ex] = v;
+    if (head) rest[n_rest + ex] = v;
     n_rest += cnt;
   }
   *steps = total;
@@ -328,18 +338,31 @@ enum { kModeRwr = 0, kModePairs = 1, kModeNs = 2 };
 // around seeds_k[g]; both budgets come from seeds[g]'s degree.  kModeNs: the node set is ns_expand's from seeds[g] /
 // seeds_k[g] (dyn smem: its V, F and S, ns_cap = cap_n); a view over cap_n vertices is counted node_cap + 1 vertices,
 // no edges, so that batch_offsets_kernel publishes the view empty.  The arguments after `flags` are unused by kModeRwr.
-template <int kMode>
-__global__ void __launch_bounds__(GCCB_ST)
-rwr_walk_unique_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices, int64_t n_nodes,
-                       const int32_t* __restrict__ budget_table, int budget_table_len,
-                       uint32_t restart_thresh, uint64_t key, const int64_t* __restrict__ seeds,
-                       const int64_t* __restrict__ sample_ids, int B, int cap_n,
-                       int32_t* __restrict__ subv_scratch, int32_t* __restrict__ subdeg_scratch,
-                       int32_t* __restrict__ rowstart_scratch, int32_t* __restrict__ pool, int pool_cap,
-                       unsigned long long* __restrict__ pool_counter,
-                       int64_t* __restrict__ counters, int32_t* __restrict__ flags,
-                       const int64_t* __restrict__ seeds_k, int ns_hops, int ns_k, int node_cap) {
-  GCCB_DYN_SMEM(int, keys);
+//
+// Wide ego-nets (walk budget > GCCB_WALK_BUDGET_MAX: their trace does not fit the CTA's keys[]).  The walk CTA of such
+// a slot only writes subv[0] = -1 and leaves it to rwr_walk_wide_kernel, whose GCCB_WIDE_CTAS CTAs claim the slots in
+// turn and run the same walk, sort and unique on a key array of their own in global memory.  The node set then moves to
+// a region of its view (WideWs), where induction reads it in place of the shared-memory copy; its offset there is
+// parked in the slot's subv[1] for induce_fill_wide_kernel.
+struct WideWs {
+  int32_t* subv;                  // [2][region]: node sets of the view's wide ego-nets, back to back
+  int32_t* subdeg;                // [2][region]
+  int32_t* rowstart;              // [2][region]
+  unsigned long long* used;       // [2] entries of each view's region claimed so far
+  unsigned* next;                 // next slot for a wide walk CTA to claim
+  int region;
+};
+
+template <int kMode, bool kWide>
+__device__ __forceinline__ void
+walk_slot(const int slot, int* keys, const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices,
+          int64_t n_nodes, const int32_t* __restrict__ budget_table, int budget_table_len, uint32_t restart_thresh,
+          uint64_t key, const int64_t* __restrict__ seeds, const int64_t* __restrict__ sample_ids, int B, int cap_n,
+          int32_t* __restrict__ subv_scratch, int32_t* __restrict__ subdeg_scratch,
+          int32_t* __restrict__ rowstart_scratch, int32_t* __restrict__ pool, int pool_cap,
+          unsigned long long* __restrict__ pool_counter, int64_t* __restrict__ counters,
+          int32_t* __restrict__ flags, const int64_t* __restrict__ seeds_k, int ns_hops, int ns_k, int node_cap,
+          const WideWs& wide) {
   __shared__ int scan_scratch[33];
   __shared__ int stage[GCCB_SW][GCCB_HIT_STAGE];      // per-warp parking of one row's hits
   __shared__ int s_tstar, s_m;
@@ -348,8 +371,7 @@ rwr_walk_unique_kernel(const int64_t* __restrict__ indptr, const int32_t* __rest
   __shared__ unsigned bloom[GCCB_BLOOM_WORDS];        // one-hash membership filter of the frontier (8 KB)
   __shared__ int hub_rows[GCCB_HUB_LIST];             // hub rows of this ego-net: probed by the whole CTA
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int slot = blockIdx.x;            // view-major: slot = view * B + g
-  const int view = slot / B, g = slot - view * B;
+  const int view = slot / B, g = slot - view * B;    // view-major: slot = view * B + g
   int64_t seed64 = seeds[g];
   seed64 = seed64 < 0 ? 0 : (seed64 >= n_nodes ? n_nodes - 1 : seed64);   // caller-supplied seeds: never read out of bounds
   const int64_t q64 = seed64;
@@ -362,6 +384,8 @@ rwr_walk_unique_kernel(const int64_t* __restrict__ indptr, const int32_t* __rest
   const int seed = (int)seed64;
   const uint64_t sample = (uint64_t)sample_ids[g];
   int32_t* subv = subv_scratch + (size_t)slot * cap_n;
+  int32_t* subdeg = subdeg_scratch + (size_t)slot * cap_n;
+  int32_t* rowstart = rowstart_scratch + (size_t)slot * cap_n;
   if (tid == 0) { s_m = 0; s_sumdeg = 0ull; }
   int n, total = 0;                                       // total: counters[2] (walk steps / ns layers expanded)
   if constexpr (kMode == kModeNs) {
@@ -381,12 +405,47 @@ rwr_walk_unique_kernel(const int64_t* __restrict__ indptr, const int32_t* __rest
   } else {
     const int64_t sdeg = indptr[q64 + 1] - indptr[q64];   // the budget's seed: the q view's
     const int budget = budget_table[sdeg < budget_table_len ? (int)sdeg : budget_table_len - 1];
+    if constexpr (!kWide) {
+      if (budget > GCCB_WALK_BUDGET_MAX) {               // rwr_walk_wide_kernel's
+        if (tid == 0) subv[0] = -1;
+        return;
+      }
+    }
     n = rwr_node_set(indptr, indices, budget, restart_thresh, key, sample, view, seed64, seed, keys, scan_scratch,
-                     &s_tstar, &s_m, flags, subv, &total);
+                     &s_tstar, &s_m, flags, kWide ? keys : subv + 1, &total);
   }
-  if (tid == 0) subv[0] = seed;
-  __syncthreads();                       // global writes of this block visible to the block
-  for (int i = tid; i < n; i += GCCB_ST) keys[i] = subv[i];
+  if constexpr (kWide) {
+    // room for the node set in the view's region.  None left: the view overflows (gccb_sample_batch_workspace), so
+    // the ego-net is only counted, its m as n - 1, a lower bound (every vertex but the seed was entered through an
+    // edge inside the ego-net), which keeps the view's edge total above what the region's size allows.
+    if (tid == 0) {
+      const unsigned long long off = atomicAdd(wide.used + view, (unsigned long long)n);
+      s_pos = off + (unsigned long long)n <= (unsigned long long)wide.region ? (int)off : -1;
+      subv[1] = s_pos;
+    }
+    __syncthreads();                                     // also: the node set in keys[] visible to the block
+    const int off = s_pos;
+    if (off < 0) {
+      if (tid == 0) {
+        counters[(size_t)slot * 4 + 0] = n;
+        counters[(size_t)slot * 4 + 1] = n - 1;
+        counters[(size_t)slot * 4 + 2] = total;
+        counters[(size_t)slot * 4 + 3] = 0;
+      }
+      return;
+    }
+    const size_t at = (size_t)view * wide.region + off;
+    subv = wide.subv + at;
+    subdeg = wide.subdeg + at;
+    rowstart = wide.rowstart + at;
+    for (int i = tid; i < n - 1; i += GCCB_ST) subv[1 + i] = keys[i];
+    if (tid == 0) subv[0] = seed;
+    keys = subv;                                         // induction reads the node set where it is
+  } else {
+    if (tid == 0) subv[0] = seed;
+    __syncthreads();                     // global writes of this block visible to the block
+    for (int i = tid; i < n; i += GCCB_ST) keys[i] = subv[i];
+  }
   for (int i = tid; i < GCCB_BLOOM_WORDS; i += GCCB_ST) bloom[i] = 0u;
   __syncthreads();
   // 99 % of the scanned neighbours are not in the ego-net: one shared-memory load rejects them, only the
@@ -400,8 +459,6 @@ rwr_walk_unique_kernel(const int64_t* __restrict__ indptr, const int32_t* __rest
   // ---- phase D: induced neighbours of every ego-net vertex (warp per vertex), ONE look at each list ------
   // Hits (local ids, in the order a scan of adj(v) meets them) are parked per warp, then moved to a slot of
   // the scratch pool claimed with one atomic per row; the fill kernel copies pool -> batched CSR.
-  int32_t* subdeg = subdeg_scratch + (size_t)slot * cap_n;
-  int32_t* rowstart = rowstart_scratch + (size_t)slot * cap_n;
   int* wstage = stage[warp];
   const unsigned lt_mask = (1u << lane) - 1u;
   int m_local = 0;
@@ -581,6 +638,52 @@ rwr_walk_unique_kernel(const int64_t* __restrict__ indptr, const int32_t* __rest
   }
 }
 
+template <int kMode>
+__global__ void __launch_bounds__(GCCB_ST)
+rwr_walk_unique_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices, int64_t n_nodes,
+                       const int32_t* __restrict__ budget_table, int budget_table_len,
+                       uint32_t restart_thresh, uint64_t key, const int64_t* __restrict__ seeds,
+                       const int64_t* __restrict__ sample_ids, int B, int cap_n,
+                       int32_t* __restrict__ subv_scratch, int32_t* __restrict__ subdeg_scratch,
+                       int32_t* __restrict__ rowstart_scratch, int32_t* __restrict__ pool, int pool_cap,
+                       unsigned long long* __restrict__ pool_counter,
+                       int64_t* __restrict__ counters, int32_t* __restrict__ flags,
+                       const int64_t* __restrict__ seeds_k, int ns_hops, int ns_k, int node_cap) {
+  GCCB_DYN_SMEM(int, keys);
+  walk_slot<kMode, false>(blockIdx.x, keys, indptr, indices, n_nodes, budget_table, budget_table_len, restart_thresh,
+                          key, seeds, sample_ids, B, cap_n, subv_scratch, subdeg_scratch, rowstart_scratch, pool,
+                          pool_cap, pool_counter, counters, flags, seeds_k, ns_hops, ns_k, node_cap, WideWs{});
+}
+
+// Pass 1 of the wide ego-nets (kModeRwr / kModePairs), after rwr_walk_unique_kernel.  grid = min(2B, GCCB_WIDE_CTAS),
+// block = GCCB_ST, no dynamic shared memory: CTA c walks in wide_keys[c][keys_len] (keys_len = pow2 >= max_budget +
+// HOPCAP) and claims slots one by one, taking those whose walk CTA left them (subv[0] = -1).
+template <int kMode>
+__global__ void __launch_bounds__(GCCB_ST)
+rwr_walk_wide_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices, int64_t n_nodes,
+                     const int32_t* __restrict__ budget_table, int budget_table_len,
+                     uint32_t restart_thresh, uint64_t key, const int64_t* __restrict__ seeds,
+                     const int64_t* __restrict__ sample_ids, int B, int cap_n,
+                     int32_t* __restrict__ subv_scratch, int32_t* __restrict__ pool, int pool_cap,
+                     unsigned long long* __restrict__ pool_counter,
+                     int64_t* __restrict__ counters, int32_t* __restrict__ flags,
+                     const int64_t* __restrict__ seeds_k, WideWs wide, int32_t* __restrict__ wide_keys,
+                     size_t keys_len) {
+  __shared__ int s_slot;
+  int* keys = wide_keys + (size_t)blockIdx.x * keys_len;
+  for (;;) {
+    if (threadIdx.x == 0) s_slot = (int)atomicAdd(wide.next, 1u);
+    __syncthreads();
+    const int slot = s_slot;
+    if (slot >= 2 * B) return;
+    if (subv_scratch[(size_t)slot * cap_n] < 0)
+      walk_slot<kMode, true>(slot, keys, indptr, indices, n_nodes, budget_table, budget_table_len, restart_thresh,
+                             key, seeds, sample_ids, B, cap_n, subv_scratch, nullptr, nullptr, pool, pool_cap,
+                             pool_counter, counters, flags, seeds_k, 0, 0, 0, wide);
+    __syncthreads();                                     // s_slot and walk_slot's shared words: next slot's
+  }
+}
+
 // Pass 2: per-view exclusive scans of n and m -> node_off / edge_off.  grid = 2, block = 256.
 __global__ void __launch_bounds__(256)
 batch_offsets_kernel(const int64_t* __restrict__ counters, int B, int node_cap, int edge_cap,
@@ -618,34 +721,29 @@ batch_offsets_kernel(const int64_t* __restrict__ counters, int B, int node_cap, 
   }
 }
 
-// Pass 3: fill the batched CSR.  grid = 2B, block = GCCB_ST, dyn smem keys[P].
-__global__ void __launch_bounds__(GCCB_ST)
-induce_fill_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices,
-                   const int64_t* __restrict__ counters, int B, int cap_n, int node_cap,
-                   int edge_cap, const int32_t* __restrict__ subv_scratch,
-                   const int32_t* __restrict__ subdeg_scratch, const int32_t* __restrict__ rowstart_scratch,
-                   const int32_t* __restrict__ pool,
-                   int32_t* __restrict__ node_off, const int32_t* __restrict__ edge_off,
-                   int32_t* __restrict__ out_indptr, int32_t* __restrict__ out_indices,
-                   int32_t* __restrict__ out_subdeg, int32_t* __restrict__ out_graph_id,
-                   int32_t* __restrict__ out_orig_id) {
-  GCCB_DYN_SMEM(int, keys);
+// Pass 3: fill the batched CSR of one ego-net.  keys: its node set, a shared-memory copy of subv made here, or (kWide)
+// subv itself.
+template <bool kWide>
+__device__ __forceinline__ void
+fill_slot(const int slot, int* keys, const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices,
+          const int64_t* __restrict__ counters, int B, int node_cap, int edge_cap, const int32_t* __restrict__ subv,
+          const int32_t* __restrict__ subdeg, const int32_t* __restrict__ rowstart, const int32_t* __restrict__ pool,
+          int32_t* __restrict__ node_off, const int32_t* __restrict__ edge_off, int32_t* __restrict__ out_indptr,
+          int32_t* __restrict__ out_indices, int32_t* __restrict__ out_subdeg, int32_t* __restrict__ out_graph_id,
+          int32_t* __restrict__ out_orig_id) {
   __shared__ int scan_scratch[33];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int slot = blockIdx.x;
   const int view = slot / B, g = slot - view * B;
   const int Nv = node_off[view * (B + 1) + B];
   if (Nv < 0) return;                                   // view overflowed: published empty
   const int n = (int)counters[(size_t)slot * 4 + 0];
   const int noff = node_off[view * (B + 1) + g];
   const int eoff = edge_off[view * (B + 1) + g];
-  const int32_t* subv = subv_scratch + (size_t)slot * cap_n;
-  const int32_t* subdeg = subdeg_scratch + (size_t)slot * cap_n;
-  const int32_t* rowstart = rowstart_scratch + (size_t)slot * cap_n;
   int32_t* v_indptr = out_indptr + (size_t)view * (node_cap + 1);
   int32_t* v_indices = out_indices + (size_t)view * edge_cap;
   const size_t nb = (size_t)view * node_cap;
-  for (int i = tid; i < n; i += GCCB_ST) keys[i] = subv[i];
+  if constexpr (!kWide)
+    for (int i = tid; i < n; i += GCCB_ST) keys[i] = subv[i];
   const int seed = subv[0];
   // row starts (view-local edge positions) = eoff + exclusive scan of induced degrees
   int run = 0;
@@ -705,6 +803,45 @@ induce_fill_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict
   }
 }
 
+// grid = 2B, block = GCCB_ST, dyn smem keys[P]
+__global__ void __launch_bounds__(GCCB_ST)
+induce_fill_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices,
+                   const int64_t* __restrict__ counters, int B, int cap_n, int node_cap,
+                   int edge_cap, const int32_t* __restrict__ subv_scratch,
+                   const int32_t* __restrict__ subdeg_scratch, const int32_t* __restrict__ rowstart_scratch,
+                   const int32_t* __restrict__ pool,
+                   int32_t* __restrict__ node_off, const int32_t* __restrict__ edge_off,
+                   int32_t* __restrict__ out_indptr, int32_t* __restrict__ out_indices,
+                   int32_t* __restrict__ out_subdeg, int32_t* __restrict__ out_graph_id,
+                   int32_t* __restrict__ out_orig_id) {
+  GCCB_DYN_SMEM(int, keys);
+  const int slot = blockIdx.x;
+  const size_t at = (size_t)slot * cap_n;
+  if (subv_scratch[at] < 0) return;                     // a wide ego-net: induce_fill_wide_kernel's
+  fill_slot<false>(slot, keys, indptr, indices, counters, B, node_cap, edge_cap, subv_scratch + at,
+                   subdeg_scratch + at, rowstart_scratch + at, pool, node_off, edge_off, out_indptr, out_indices,
+                   out_subdeg, out_graph_id, out_orig_id);
+}
+
+// Pass 3 of the wide ego-nets, after induce_fill_kernel.  grid = 2B, block = GCCB_ST, no dynamic shared memory: the
+// CTA of a slot that rwr_walk_wide_kernel induced fills it from the view's region.
+__global__ void __launch_bounds__(GCCB_ST)
+induce_fill_wide_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices,
+                        const int64_t* __restrict__ counters, int B, int cap_n, int node_cap, int edge_cap,
+                        const int32_t* __restrict__ subv_scratch, WideWs wide, const int32_t* __restrict__ pool,
+                        int32_t* __restrict__ node_off, const int32_t* __restrict__ edge_off,
+                        int32_t* __restrict__ out_indptr, int32_t* __restrict__ out_indices,
+                        int32_t* __restrict__ out_subdeg, int32_t* __restrict__ out_graph_id,
+                        int32_t* __restrict__ out_orig_id) {
+  const int slot = blockIdx.x;
+  const int32_t* mark = subv_scratch + (size_t)slot * cap_n;
+  if (mark[0] >= 0 || mark[1] < 0) return;             // an ordinary slot, or one without room (its view overflowed)
+  const size_t at = (size_t)(slot / B) * wide.region + mark[1];
+  fill_slot<true>(slot, wide.subv + at, indptr, indices, counters, B, node_cap, edge_cap, wide.subv + at,
+                  wide.subdeg + at, wide.rowstart + at, pool, node_off, edge_off, out_indptr, out_indices,
+                  out_subdeg, out_graph_id, out_orig_id);
+}
+
 // One thread per sample: step ~ step_dist (first index with cdf > u, 53 Philox bits, GCCB_TAG_STEP), then `step`
 // uniform hops of a plain walk from seeds_q[i] (hop h: GCCB_TAG_KHOP, hop field h).  A vertex without neighbours ends
 // the walk where it is.
@@ -752,11 +889,95 @@ extern "C" int gccb_draw_seeds(const double* cdf, int64_t n_nodes, uint64_t key,
 }
 
 // workspace layout: subv[2B][cap_n] | subdeg[2B][cap_n] | rowstart[2B][cap_n] | pool counter (16 ints) | pool[2*edge_cap]
+// and, when max_budget > GCCB_WALK_BUDGET_MAX (cap_n then that of GCCB_WALK_BUDGET_MAX):
+//   | wide subv[2][R] | wide subdeg[2][R] | wide rowstart[2][R] | wide keys[min(2B, GCCB_WIDE_CTAS)][pow2 >= max_budget + HOPCAP]
+// with R = min(edge_cap + B, 2^31 - 1).  The 16 ints hold the pool counter, the next wide slot and each view's R used.
 static int sampler_cap_n(int max_budget) { return (max_budget + (int)GCCB_HOPCAP + 1 + 3) & ~3; }
+static bool sampler_wide(int max_budget) { return max_budget > GCCB_WALK_BUDGET_MAX; }
+static int wide_region(int batch, int edge_cap) {
+  const long long r = (long long)edge_cap + batch;
+  return (int)(r < 0x7fffffffll ? r : 0x7fffffffll);
+}
+static int wide_ctas(int batch) { return 2 * batch < GCCB_WIDE_CTAS ? 2 * batch : GCCB_WIDE_CTAS; }
+static size_t wide_keys_len(int max_budget) {
+  size_t p = 1;
+  while (p < (size_t)max_budget + GCCB_HOPCAP) p <<= 1;
+  return p;
+}
 
 extern "C" size_t gccb_sample_batch_workspace(int32_t batch, int32_t max_budget, int32_t edge_cap) {
-  return ((size_t)3 * (size_t)(2 * batch) * (size_t)sampler_cap_n(max_budget) + 16 + (size_t)2 * (size_t)edge_cap) *
-         sizeof(int32_t);
+  const bool wide = sampler_wide(max_budget);
+  const int cap_n = sampler_cap_n(wide ? GCCB_WALK_BUDGET_MAX : max_budget);
+  size_t ints = (size_t)3 * (size_t)(2 * batch) * (size_t)cap_n + 16 + (size_t)2 * (size_t)edge_cap;
+  if (wide)
+    ints += (size_t)6 * (size_t)wide_region(batch, edge_cap) + (size_t)wide_ctas(batch) * wide_keys_len(max_budget);
+  return ints * sizeof(int32_t);
+}
+
+// gccb_sample_batch (kModeRwr: seeds_k unused) and gccb_sample_batch_pairs (kModePairs)
+template <int kMode>
+static int sample_batch_rwr(const char* what, const gccb_graph_t* graph, const int64_t* seeds, const int64_t* seeds_k,
+                            const int64_t* sample_ids, const gccb_batch_t* batch, void* workspace,
+                            size_t workspace_bytes, gccb_stream_t stream) {
+  const int B = batch->batch;
+  const bool wide = sampler_wide(graph->max_budget);
+  if (wide && wide_keys_len(graph->max_budget) > (size_t)GCCB_WIDE_KEYS_MAX) {
+    set_last_error("%s: walk budget %d: a trace of up to %d vertices does not fit int32 positions", what,
+                   graph->max_budget, graph->max_budget + (int)GCCB_HOPCAP - 1);
+    return GCCB_ERR_CAPACITY;
+  }
+  const int cap_n = sampler_cap_n(wide ? GCCB_WALK_BUDGET_MAX : graph->max_budget);
+  if (workspace_bytes < gccb_sample_batch_workspace(B, graph->max_budget, batch->edge_cap)) {
+    set_last_error("%s: workspace too small", what);
+    return GCCB_ERR_CAPACITY;
+  }
+  const int P = wide ? GCCB_WALK_KEYS : pow2_ge(graph->max_budget + (int)GCCB_HOPCAP);
+  const size_t smem = (size_t)P * sizeof(int);
+  int32_t* subv = (int32_t*)workspace;
+  int32_t* subdeg = subv + (size_t)2 * B * cap_n;
+  int32_t* rowstart = subdeg + (size_t)2 * B * cap_n;
+  unsigned long long* pool_counter = (unsigned long long*)(rowstart + (size_t)2 * B * cap_n);   // 16 ints reserved, 8-byte aligned
+  int32_t* pool = (int32_t*)pool_counter + 16;
+  // pool positions are stored per row as int32: the pool is capped below 2^31 entries (2 * edge_cap overflows
+  // an int for edge_cap > 2^30 -- the 65,536-ego-net sweep of config 5)
+  const long long want_cap = 2ll * (long long)batch->edge_cap;
+  const int pool_cap = (int)(want_cap < 0x7fff0000ll ? want_cap : 0x7fff0000ll);
+  cudaMemsetAsync(pool_counter, 0, wide ? 16 * sizeof(int32_t) : sizeof(unsigned long long), (cudaStream_t)stream);
+  auto k1 = rwr_walk_unique_kernel<kMode>;
+  auto k3 = induce_fill_kernel;
+  if (smem > 48 * 1024) {
+    gccb::ensure_dyn_smem(k1, smem);
+    gccb::ensure_dyn_smem(k3, smem);
+  }
+  GCCB_LAUNCH(k1, 2 * B, GCCB_ST, smem, stream, graph->indptr, graph->indices, graph->n_nodes, graph->budget_table,
+              graph->budget_table_len, graph->restart_thresh, graph->key, seeds, sample_ids, B,
+              cap_n, subv, subdeg, rowstart, pool, pool_cap, pool_counter, batch->counters, batch->flags,
+              seeds_k, 0, 0, 0);
+  WideWs ww = {};
+  if (wide) {
+    ww.region = wide_region(B, batch->edge_cap);
+    ww.subv = pool + (size_t)2 * batch->edge_cap;
+    ww.subdeg = ww.subv + (size_t)2 * ww.region;
+    ww.rowstart = ww.subdeg + (size_t)2 * ww.region;
+    ww.used = pool_counter + 2;
+    ww.next = (unsigned*)(pool_counter + 1);
+    int32_t* wide_keys = ww.rowstart + (size_t)2 * ww.region;
+    GCCB_LAUNCH(rwr_walk_wide_kernel<kMode>, wide_ctas(B), GCCB_ST, 0, stream, graph->indptr, graph->indices,
+                graph->n_nodes, graph->budget_table, graph->budget_table_len, graph->restart_thresh, graph->key,
+                seeds, sample_ids, B, cap_n, subv, pool, pool_cap, pool_counter, batch->counters, batch->flags,
+                seeds_k, ww, wide_keys, wide_keys_len(graph->max_budget));
+  }
+  GCCB_LAUNCH(batch_offsets_kernel, 2, 256, 0, stream, batch->counters, B, batch->node_cap,
+              batch->edge_cap, batch->node_off, batch->edge_off, batch->flags);
+  GCCB_LAUNCH(k3, 2 * B, GCCB_ST, smem, stream, graph->indptr, graph->indices, batch->counters, B,
+              cap_n, batch->node_cap, batch->edge_cap, subv, subdeg, rowstart, pool, batch->node_off,
+              batch->edge_off, batch->indptr, batch->indices, batch->sub_deg, batch->graph_id,
+              batch->orig_id);
+  if (wide)
+    GCCB_LAUNCH(induce_fill_wide_kernel, 2 * B, GCCB_ST, 0, stream, graph->indptr, graph->indices, batch->counters,
+                B, cap_n, batch->node_cap, batch->edge_cap, subv, ww, pool, batch->node_off, batch->edge_off,
+                batch->indptr, batch->indices, batch->sub_deg, batch->graph_id, batch->orig_id);
+  return check_launch(what);
 }
 
 extern "C" int gccb_sample_batch(const gccb_graph_t* graph, const int64_t* seeds,
@@ -767,46 +988,8 @@ extern "C" int gccb_sample_batch(const gccb_graph_t* graph, const int64_t* seeds
     set_last_error("gccb_sample_batch: bad argument");
     return GCCB_ERR_BADARG;
   }
-  const int B = batch->batch;
-  const int cap_n = sampler_cap_n(graph->max_budget);
-  if (workspace_bytes < gccb_sample_batch_workspace(B, graph->max_budget, batch->edge_cap)) {
-    set_last_error("gccb_sample_batch: workspace too small");
-    return GCCB_ERR_CAPACITY;
-  }
-  const int P = pow2_ge(graph->max_budget + (int)GCCB_HOPCAP);
-  const size_t smem = (size_t)P * sizeof(int);
-  if (smem > 200 * 1024) {
-    set_last_error("gccb_sample_batch: walk budget %d needs %zu B of shared memory (> 200 KiB)",
-                   graph->max_budget, smem);
-    return GCCB_ERR_CAPACITY;
-  }
-  int32_t* subv = (int32_t*)workspace;
-  int32_t* subdeg = subv + (size_t)2 * B * cap_n;
-  int32_t* rowstart = subdeg + (size_t)2 * B * cap_n;
-  unsigned long long* pool_counter = (unsigned long long*)(rowstart + (size_t)2 * B * cap_n);   // 16 ints reserved, 8-byte aligned
-  int32_t* pool = (int32_t*)pool_counter + 16;
-  // pool positions are stored per row as int32: the pool is capped below 2^31 entries (2 * edge_cap overflows
-  // an int for edge_cap > 2^30 -- the 65,536-ego-net sweep of config 5)
-  const long long want_cap = 2ll * (long long)batch->edge_cap;
-  const int pool_cap = (int)(want_cap < 0x7fff0000ll ? want_cap : 0x7fff0000ll);
-  cudaMemsetAsync(pool_counter, 0, sizeof(unsigned long long), (cudaStream_t)stream);
-  auto k1 = rwr_walk_unique_kernel<kModeRwr>;
-  auto k3 = induce_fill_kernel;
-  if (smem > 48 * 1024) {
-    gccb::ensure_dyn_smem(k1, smem);
-    gccb::ensure_dyn_smem(k3, smem);
-  }
-  GCCB_LAUNCH(k1, 2 * B, GCCB_ST, smem, stream, graph->indptr, graph->indices, graph->n_nodes, graph->budget_table,
-              graph->budget_table_len, graph->restart_thresh, graph->key, seeds, sample_ids, B,
-              cap_n, subv, subdeg, rowstart, pool, pool_cap, pool_counter, batch->counters, batch->flags,
-              (const int64_t*)nullptr, 0, 0, 0);
-  GCCB_LAUNCH(batch_offsets_kernel, 2, 256, 0, stream, batch->counters, B, batch->node_cap,
-              batch->edge_cap, batch->node_off, batch->edge_off, batch->flags);
-  GCCB_LAUNCH(k3, 2 * B, GCCB_ST, smem, stream, graph->indptr, graph->indices, batch->counters, B,
-              cap_n, batch->node_cap, batch->edge_cap, subv, subdeg, rowstart, pool, batch->node_off,
-              batch->edge_off, batch->indptr, batch->indices, batch->sub_deg, batch->graph_id,
-              batch->orig_id);
-  return check_launch("gccb_sample_batch");
+  return sample_batch_rwr<kModeRwr>("gccb_sample_batch", graph, seeds, (const int64_t*)nullptr, sample_ids, batch,
+                                    workspace, workspace_bytes, stream);
 }
 
 // ---- the reference's other views: k-hop key seeds (step_dist) and neighbour sampling (aug="ns") ----------------
@@ -834,44 +1017,8 @@ extern "C" int gccb_sample_batch_pairs(const gccb_graph_t* graph, const int64_t*
     set_last_error("gccb_sample_batch_pairs: bad argument");
     return GCCB_ERR_BADARG;
   }
-  const int B = batch->batch;
-  const int cap_n = sampler_cap_n(graph->max_budget);
-  if (workspace_bytes < gccb_sample_batch_workspace(B, graph->max_budget, batch->edge_cap)) {
-    set_last_error("gccb_sample_batch_pairs: workspace too small");
-    return GCCB_ERR_CAPACITY;
-  }
-  const int P = pow2_ge(graph->max_budget + (int)GCCB_HOPCAP);
-  const size_t smem = (size_t)P * sizeof(int);
-  if (smem > 200 * 1024) {
-    set_last_error("gccb_sample_batch_pairs: walk budget %d needs %zu B of shared memory (> 200 KiB)",
-                   graph->max_budget, smem);
-    return GCCB_ERR_CAPACITY;
-  }
-  int32_t* subv = (int32_t*)workspace;
-  int32_t* subdeg = subv + (size_t)2 * B * cap_n;
-  int32_t* rowstart = subdeg + (size_t)2 * B * cap_n;
-  unsigned long long* pool_counter = (unsigned long long*)(rowstart + (size_t)2 * B * cap_n);
-  int32_t* pool = (int32_t*)pool_counter + 16;
-  const long long want_cap = 2ll * (long long)batch->edge_cap;
-  const int pool_cap = (int)(want_cap < 0x7fff0000ll ? want_cap : 0x7fff0000ll);
-  cudaMemsetAsync(pool_counter, 0, sizeof(unsigned long long), (cudaStream_t)stream);
-  auto k1 = rwr_walk_unique_kernel<kModePairs>;
-  auto k3 = induce_fill_kernel;
-  if (smem > 48 * 1024) {
-    gccb::ensure_dyn_smem(k1, smem);
-    gccb::ensure_dyn_smem(k3, smem);
-  }
-  GCCB_LAUNCH(k1, 2 * B, GCCB_ST, smem, stream, graph->indptr, graph->indices, graph->n_nodes, graph->budget_table,
-              graph->budget_table_len, graph->restart_thresh, graph->key, seeds_q, sample_ids, B,
-              cap_n, subv, subdeg, rowstart, pool, pool_cap, pool_counter, batch->counters, batch->flags,
-              seeds_k, 0, 0, 0);
-  GCCB_LAUNCH(batch_offsets_kernel, 2, 256, 0, stream, batch->counters, B, batch->node_cap,
-              batch->edge_cap, batch->node_off, batch->edge_off, batch->flags);
-  GCCB_LAUNCH(k3, 2 * B, GCCB_ST, smem, stream, graph->indptr, graph->indices, batch->counters, B,
-              cap_n, batch->node_cap, batch->edge_cap, subv, subdeg, rowstart, pool, batch->node_off,
-              batch->edge_off, batch->indptr, batch->indices, batch->sub_deg, batch->graph_id,
-              batch->orig_id);
-  return check_launch("gccb_sample_batch_pairs");
+  return sample_batch_rwr<kModePairs>("gccb_sample_batch_pairs", graph, seeds_q, seeds_k, sample_ids, batch,
+                                      workspace, workspace_bytes, stream);
 }
 
 // shared memory of an ns ego-net of cap vertices: V[cap] | F[cap] | S[pow2 >= max(k, 2) * cap]

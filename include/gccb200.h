@@ -106,7 +106,16 @@ int gccb_draw_seeds(const double* cdf, int64_t n_nodes, uint64_t key, int64_t fi
  * dgl.contrib.sampling.random_walk_with_restart (graph_dataset.py:125-130),
  * _rwr_trace_to_dgl_graph's unique/sort/subgraph (data_util.py:218-239) and
  * dgl.batch (data_util.py:29) for both views of `batch->batch` samples.
- * seeds/sample_ids: [B] (both views start from the same seed: step_dist=[1,0,0]).     */
+ * seeds/sample_ids: [B] (both views start from the same seed: step_dist=[1,0,0]).
+ * Workspace, in int32 words, with cap(b) = (b + 65 + 3) & ~3:
+ *   max_budget <= 32704:  3 * 2B * cap(max_budget) + 16 + 2 * edge_cap
+ *   above (wide path):    3 * 2B * cap(32704) + 16 + 2 * edge_cap + 6 * R + min(2B, 32) * K
+ *     R = min(edge_cap + B, 2^31 - 1)  per view and array, the node sets and rows of the view's wide ego-nets (an RWR
+ *                                      ego-net has m >= n - 1, so a view holding more overflows edge_cap anyway),
+ *     K = pow2 >= max_budget + 64      the trace of one of the (at most 32) wide walk CTAs in flight.
+ * A sample whose budget exceeds 32,704 (its trace does not fit the walk CTA's 128 KiB of shared memory) is walked,
+ * sorted and induced from global memory by the wide kernels, selected per sample on the device; outputs are the
+ * same.  max_budget + 64 above 2^30 (int32 trace positions) is refused with GCCB_ERR_CAPACITY.                  */
 size_t gccb_sample_batch_workspace(int32_t batch, int32_t max_budget, int32_t edge_cap);
 int gccb_sample_batch(const gccb_graph_t* graph, const int64_t* seeds,
                       const int64_t* sample_ids, const gccb_batch_t* batch, void* workspace,
