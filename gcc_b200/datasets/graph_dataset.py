@@ -206,16 +206,21 @@ class BatchBuffers:
         f = int(self.flags.item())
         if f:
             self.flags.zero_()
-            if f & _capi.FLAG_EIG_NOCONV:
-                self.eig_noconv_events = getattr(self, "eig_noconv_events", 0) + 1
-                if self.eig_noconv_events == 1:
-                    import warnings
-                    warnings.warn("gcc_b200: an ego-net eigensolve hit its iteration limit "
-                                  "(residual above 2.5e-4); features kept as is")
-                f &= ~_capi.FLAG_EIG_NOCONV
-            if f:
-                raise _lib.GccbError("device flags: " + "; ".join(
-                    n for b, n in _capi.FLAG_NAMES.items() if f & b))
+            self.raise_flags(f)
+
+    def raise_flags(self, f, where=""):
+        """Interpret a flag word already read from these buffers: warn once on eigensolver non-convergence, raise
+        GccbError (prefixed by `where`) on any other flag."""
+        if f & _capi.FLAG_EIG_NOCONV:
+            self.eig_noconv_events = getattr(self, "eig_noconv_events", 0) + 1
+            if self.eig_noconv_events == 1:
+                import warnings
+                warnings.warn("gcc_b200: an ego-net eigensolve hit its iteration limit "
+                              "(residual above 2.5e-4); features kept as is")
+            f &= ~_capi.FLAG_EIG_NOCONV
+        if f:
+            raise _lib.GccbError(where + "device flags: " + "; ".join(
+                n for b, n in _capi.FLAG_NAMES.items() if f & b))
 
 
 def step_cdf(step_dist):
@@ -230,8 +235,9 @@ def step_cdf(step_dist):
     return np.ascontiguousarray(cdf / cdf[-1])
 
 
-def sample_pairs(ds, buf, first_sample, seeds=None):
-    """Both views of buf's B pairs with sample ids first_sample.., walked on ds.graph with no host sync.  Seeds: drawn
+def sample_pairs(ds, buf, first_sample, seeds=None, sample_ids=None):
+    """Both views of buf's B pairs with sample ids first_sample.. (or `sample_ids`, device int64 [B], with given
+    seeds), walked on ds.graph with no host sync.  Seeds: drawn
     (gccb_draw_seeds), or `seeds` (device int64 [B], or buf.seeds already written).  Views: by ds.step_cdf (None: the
     k view shares the seed; else gccb_pair_seeds draws buf.seeds_k) and ds.aug ("rwr": gccb_sample_batch, or
     gccb_sample_batch_pairs for separate seeds; "ns": gccb_ns_batch).  Returns buf."""
@@ -242,7 +248,10 @@ def sample_pairs(ds, buf, first_sample, seeds=None):
     else:
         if seeds is not buf.seeds:
             buf.seeds.copy_(seeds, non_blocking=True)
-        torch.arange(first_sample, first_sample + buf.B, device=buf.seeds.device, out=buf.sample_ids)
+        if sample_ids is not None:
+            buf.sample_ids.copy_(sample_ids, non_blocking=True)
+        else:
+            torch.arange(first_sample, first_sample + buf.B, device=buf.seeds.device, out=buf.sample_ids)
     cdf, aug = getattr(ds, "step_cdf", None), getattr(ds, "aug", "rwr")   # the labeled datasets: the defaults
     seeds_k = buf.seeds
     if cdf is not None:

@@ -10,20 +10,32 @@ the nodes go through in `--batch-size` chunks -- eval-mode encoding is per-graph
 the same.
 
 `--dataset` is one of the reference's downstream datasets, read from ./data as the reference reads them
-(datasets/downstream.py), an .npz CSR (indptr, indices) or `synthetic-<kind>`:
+(datasets/downstream.py), an .npz CSR (indptr, indices), a DGL .bin corpus or `synthetic-<kind>`:
   - node datasets (airports and h-index from data/struc2vec, data/hindex; kdd ... icde from data/panther): the
     multigraph of the reference's _create_dgl_graph, parallel edges kept, one row per node;
+  - .bin corpora (datasets/dgl_bin.py, as train.py and x2dgl read and write them): one row per vertex of the union
+    of the file's graphs, in file order (the ids load_graphs assigns);
   - graph datasets (the five TU sets from data/<NAME>): q and k are both the whole graph with the seed on its first
     maximum-degree vertex (entire_graph=True), so the row of a graph is the encoding of that whole graph.
+
+Node rows go through gcc_b200.embed.EmbedEngine (the data path of `--prefetch` batches runs ahead of the encoder;
+`--prefetch 0` is the serial loop) straight into the .npy file through a memmap, so host memory does not grow with
+the graph.  `--nodes FILE` writes only the rows of the listed ids, in the file's order.  `--gpu 0 1 ...` splits the
+rows into one contiguous, batch-aligned shard per entry, each embedded by its own process on that device and written
+at its offsets in the shared file; the same id may repeat.  A row depends only on (run seed, node id), so the shards
+exchange nothing.
 """
 import argparse
+import multiprocessing
+import multiprocessing.connection
 import os
+import traceback
 
 import numpy as np
 import torch
 
 from gcc_b200.datasets import downstream, synthetic
-from gcc_b200.datasets.graph_dataset import NodeClassificationDataset
+from gcc_b200.datasets.graph_dataset import NodeClassificationDataset, load_graphs
 from gcc_b200.datasets.labeled import GraphClassificationDatasetLabeled
 from gcc_b200.models import GraphEncoder
 
@@ -36,6 +48,7 @@ ENCODER_KWARGS = {
     "num_layers": "num_layer", "num_step_set2set": "set2set_iter",
     "num_layer_set2set": "set2set_lstm_layer", "gnn_model": "model", "norm": "norm",
 }
+WORKER_ERROR_CHARS = 16384                     # a worker's traceback, cut to fit the pipe without blocking
 
 
 def test_moco(train_loader, model, opt):
@@ -65,15 +78,123 @@ def test_graphs(dataset, model, opt):
 
 
 def resolve_graph(name, nodes, edges):
-    """`--dataset`: a named node dataset is read from ./data as a multigraph; an .npz path is passed through;
-    synthetic-chunglu / synthetic-er are generated."""
+    """`--dataset`: a named node dataset is read from ./data as a multigraph; an .npz or .bin path is passed
+    through; synthetic-chunglu / synthetic-er are generated."""
     if name in downstream.NODE_DSETS:
         return downstream.node_dataset_graph(name)
-    if name.endswith(".npz"):
+    if name.endswith(".npz") or name.endswith(".bin"):
         return name
     if name.endswith("chunglu"):
         return synthetic.chung_lu(nodes, edges, 0.5, seed=0)
     return synthetic.erdos_renyi(nodes, edges, seed=0)
+
+
+def parse_gpus(gpu):
+    """`--gpu`: None (device 0), one id, or a list of ids (one shard each; repeats allowed) -> list of ints."""
+    if gpu is None:
+        return [0]
+    ids = [int(g) for g in gpu] if isinstance(gpu, (list, tuple)) else [int(gpu)]
+    if not ids or min(ids) < 0:
+        raise ValueError("--gpu takes one or more device ids >= 0, got %r" % (gpu,))
+    return ids
+
+
+def read_nodes(path):
+    """`--nodes`: a .npy array or a text file of integer node ids (whitespace or newline separated) -> int64 [n]."""
+    if path.endswith(".npy"):
+        ids = np.load(path)
+        if ids.ndim != 1 or not np.issubdtype(ids.dtype, np.integer):
+            raise ValueError("%s: expected a 1-D integer array, got %s %s" % (path, ids.dtype, ids.shape))
+    else:
+        with open(path) as f:
+            tokens = f.read().split()
+        try:
+            ids = np.array([int(t) for t in tokens], dtype=np.int64)
+        except ValueError as e:
+            raise ValueError("%s: node ids must be integers (%s)" % (path, e)) from None
+    if ids.size == 0:
+        raise ValueError("%s lists no node ids" % path)
+    return ids.astype(np.int64)
+
+
+def split_shards(n, batch_size, workers):
+    """Rows 0..n-1 in batches of batch_size, split into `workers` contiguous runs of whole batches (the first
+    n_batches mod workers runs get one batch more) -> one (lo, hi) per worker; workers beyond the batch count get
+    empty runs (lo == hi)."""
+    n_b = -(-n // batch_size)
+    q, r = divmod(n_b, workers)
+    out, b0 = [], 0
+    for w in range(workers):
+        b1 = b0 + q + (w < r)
+        out.append((min(n, b0 * batch_size), min(n, b1 * batch_size)))
+        b0 = b1
+    return out
+
+
+def _node_rows(load_path, graph, batch_size, prefetch, gpu, rows, out):
+    """Embed `rows` (a range of node ids or an int64 array of them) of `graph` on device `gpu` into `out`."""
+    from gcc_b200.embed import EmbedEngine
+    torch.cuda.set_device(gpu)
+    dev = torch.device("cuda", gpu)
+    ckpt = torch.load(load_path, map_location="cpu", weights_only=False)
+    opt = ckpt["opt"]
+    encoder = GraphEncoder(degree_input=True, **{kw: getattr(opt, attr) for kw, attr in ENCODER_KWARGS.items()})
+    encoder.load_state_dict(ckpt["model"])
+    encoder = encoder.to(dev).eval()
+    del ckpt
+    nodes = NodeClassificationDataset(
+        dataset=graph, rw_hops=opt.rw_hops, subgraph_size=opt.subgraph_size, restart_prob=opt.restart_prob,
+        positional_embedding_size=opt.positional_embedding_size, device=dev, seed=getattr(opt, "seed", 0),
+        batch_size=batch_size)
+    EmbedEngine(nodes, encoder, prefetch=prefetch).run(rows, out)
+    torch.cuda.synchronize(dev)
+
+
+def _worker(load_path, dataset, graph_nodes, graph_edges, batch_size, prefetch, gpu, rows, out_file, lo, hi, errors):
+    """One shard in its own process: rows lo..hi-1 of the output file."""
+    try:
+        graph = resolve_graph(dataset, graph_nodes, graph_edges)
+        out = np.lib.format.open_memmap(out_file, mode="r+")
+        _node_rows(load_path, graph, batch_size, prefetch, gpu, rows, out[lo:hi])
+        out.flush()
+    except BaseException:
+        errors.send(traceback.format_exc()[-WORKER_ERROR_CHARS:])
+        raise SystemExit(1)
+
+
+def _run_shards(args_test, gpus, shards, rows_of, out_file, prefetch):
+    """One process per non-empty shard; all of them joined.  If one fails, the others are terminated and its error
+    is raised."""
+    ctx = multiprocessing.get_context("spawn")
+    procs = []
+    try:
+        for i, (gpu, (lo, hi)) in enumerate(zip(gpus, shards)):
+            if lo == hi:
+                continue
+            recv, send = ctx.Pipe(duplex=False)
+            p = ctx.Process(target=_worker, name="generate-shard-%d" % i,
+                            args=(args_test.load_path, args_test.dataset, args_test.graph_nodes, args_test.graph_edges,
+                                  args_test.batch_size, prefetch, gpu, rows_of(lo, hi), out_file, lo, hi, send))
+            p.start()
+            send.close()
+            procs.append((i, gpu, lo, hi, p, recv))
+        pending = [p for *_, p, _ in procs]
+        while pending:
+            multiprocessing.connection.wait([p.sentinel for p in pending])
+            for i, gpu, lo, hi, p, recv in procs:
+                if p in pending and p.exitcode is not None:
+                    pending.remove(p)
+                    if p.exitcode != 0:
+                        msg = recv.recv() if recv.poll() else "exit code %d" % p.exitcode
+                        raise RuntimeError("generate.py: shard %d (gpu %d, rows %d..%d) failed:\n%s"
+                                           % (i, gpu, lo, hi - 1, msg))
+    finally:
+        for *_, p, recv in procs:
+            if p.is_alive():
+                p.terminate()
+        for *_, p, recv in procs:
+            p.join()
+            recv.close()
 
 
 def main(args_test):
@@ -86,46 +207,79 @@ def main(args_test):
     ckpt = torch.load(path, map_location="cpu", weights_only=False)
     print("=> loaded successfully '{}' (epoch {})".format(path, ckpt["epoch"]))
     opt = ckpt["opt"]
-    gpu = args_test.gpu or 0
-    torch.cuda.set_device(gpu)
-    opt.device = torch.device("cuda", gpu)
-
-    encoder = GraphEncoder(degree_input=True, **{kw: getattr(opt, attr) for kw, attr in ENCODER_KWARGS.items()})
-    encoder.load_state_dict(ckpt["model"])
-    encoder = encoder.to(opt.device)
-    del ckpt
+    gpus = parse_gpus(getattr(args_test, "gpu", None))
+    prefetch = getattr(args_test, "prefetch", 4)
+    nodes_file = getattr(args_test, "nodes", None)
+    stem = os.path.basename(args_test.dataset)
+    stem = stem[:-4] if stem.endswith(".npz") or stem.endswith(".bin") else stem
+    out = os.path.join(getattr(opt, "model_folder", "."), stem)
 
     if args_test.dataset in downstream.GRAPH_DSETS:
+        if len(gpus) > 1 or nodes_file:
+            raise SystemExit("whole-graph datasets are embedded on one GPU, every graph: --gpu takes one id and "
+                             "--nodes does not apply")
+        torch.cuda.set_device(gpus[0])
+        opt.device = torch.device("cuda", gpus[0])
+        encoder = GraphEncoder(degree_input=True, **{kw: getattr(opt, attr) for kw, attr in ENCODER_KWARGS.items()})
+        encoder.load_state_dict(ckpt["model"])
+        encoder = encoder.to(opt.device)
+        del ckpt
         graphs = GraphClassificationDatasetLabeled(
             downstream.graph_dataset_graphs(args_test.dataset), rw_hops=opt.rw_hops,
             subgraph_size=opt.subgraph_size, restart_prob=opt.restart_prob,
             positional_embedding_size=opt.positional_embedding_size, device=opt.device,
             batch_size=args_test.batch_size)
         emb = test_graphs(graphs, encoder, opt)
-    else:
-        nodes = NodeClassificationDataset(
-            dataset=resolve_graph(args_test.dataset, args_test.graph_nodes, args_test.graph_edges),
-            rw_hops=opt.rw_hops, subgraph_size=opt.subgraph_size, restart_prob=opt.restart_prob,
-            positional_embedding_size=opt.positional_embedding_size, device=opt.device,
-            seed=getattr(opt, "seed", 0), batch_size=args_test.batch_size)
-        emb = test_moco(nodes, encoder, opt)
+        np.save(out, emb.numpy())
+        print("saved {} embeddings of dim {} to {}.npy".format(emb.shape[0], emb.shape[1], out))
+        return emb
 
-    stem = os.path.basename(args_test.dataset)
-    stem = stem[:-4] if stem.endswith(".npz") else stem
-    out = os.path.join(getattr(opt, "model_folder", "."), stem)
-    np.save(out, emb.numpy())
-    print("saved {} embeddings of dim {} to {}.npy".format(emb.shape[0], emb.shape[1], out))
-    return emb
+    del ckpt
+    graph = resolve_graph(args_test.dataset, args_test.graph_nodes, args_test.graph_edges)
+    n_nodes = load_graphs(graph)[0].num_nodes
+    ids = None
+    if nodes_file:
+        ids = read_nodes(nodes_file)
+        if ids.min() < 0 or ids.max() >= n_nodes:
+            raise SystemExit("%s: node ids must lie in 0..%d" % (nodes_file, n_nodes - 1))
+    n = n_nodes if ids is None else len(ids)
+    rows_of = (lambda lo, hi: range(lo, hi)) if ids is None else (lambda lo, hi: ids[lo:hi])
+    out_file = out + ".npy"
+    emb = np.lib.format.open_memmap(out_file, mode="w+", dtype=np.float32, shape=(n, opt.hidden_size))
+    try:
+        if len(gpus) == 1:
+            _node_rows(path, graph, args_test.batch_size, prefetch, gpus[0], rows_of(0, n), emb)
+        else:
+            # shards aligned to the batches a one-GPU run makes, so every batch holds the same nodes
+            B = min(args_test.batch_size, n_nodes)
+            _run_shards(args_test, gpus, split_shards(n, B, len(gpus)), rows_of, out_file, prefetch)
+        emb.flush()
+    except BaseException:
+        del emb
+        os.remove(out_file)
+        raise
+    print("saved {} embeddings of dim {} to {}".format(n, opt.hidden_size, out_file))
+    return torch.from_numpy(np.asarray(emb))
 
 
-if __name__ == "__main__":
+def parse_args(argv=None):
     ap = argparse.ArgumentParser("inference export: node embeddings from a pretraining checkpoint")
     ap.add_argument("--load-path", type=str, required=True, help="path to load model")
     ap.add_argument("--dataset", type=str, default="synthetic-er",
-                    help="a downstream dataset (%s; files under ./data), an .npz CSR file (indptr, indices) or "
-                         "synthetic-er / synthetic-chunglu" % ", ".join(downstream.NODE_DSETS + downstream.GRAPH_DSETS))
+                    help="a downstream dataset (%s; files under ./data), an .npz CSR file (indptr, indices), a DGL "
+                         ".bin corpus or synthetic-er / synthetic-chunglu"
+                         % ", ".join(downstream.NODE_DSETS + downstream.GRAPH_DSETS))
     ap.add_argument("--graph-nodes", type=int, default=2000, help="size of a synthetic target graph")
     ap.add_argument("--graph-edges", type=int, default=10000)
     ap.add_argument("--batch-size", type=int, default=256, help="nodes (or whole graphs) encoded per launch group")
-    ap.add_argument("--gpu", default=None, type=int, help="GPU id to use.")
-    main(ap.parse_args())
+    ap.add_argument("--gpu", default=None, type=int, nargs="+",
+                    help="GPU id(s): one shard of the rows per entry, each in its own process (repeats allowed)")
+    ap.add_argument("--prefetch", type=int, default=4,
+                    help="batches whose sampling and positional features run ahead of the encoder; 0 = serial")
+    ap.add_argument("--nodes", type=str, default=None,
+                    help="a .npy or text file of node ids: write only their rows, in the file's order")
+    return ap.parse_args(argv)
+
+
+if __name__ == "__main__":
+    main(parse_args())
