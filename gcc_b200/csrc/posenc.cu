@@ -26,8 +26,10 @@
 //      L2-resident workspace above that.
 //
 // All return an orthonormal basis of every eigenspace (degenerate clusters included), Ritz
-// values as Rayleigh quotients, a deterministic sign (largest-|.| component positive) and are
-// deterministic run to run (no floating-point atomics on the results).
+// values as Rayleigh quotients, a deterministic sign (largest-|.| component positive).  A graph's output bits depend
+// on the graph alone -- not on the run, its slot, view, batch or node_cap, nor on GCCB200_DENSE_MAX where its class
+// stays: no floating-point atomics on the results, a Philox start block keyed by (entry, n), cluster partials summed
+// in rank order, and the cluster kernel's hub-row list taken in row order.
 #include "common.cuh"
 
 #include <stdlib.h>
@@ -845,7 +847,9 @@ __device__ __forceinline__ void posenc_chfsi_item(const int item, const int32_t*
     __syncthreads();
     GCCB_TICK(5);
   }
-  if (!converged && tid == 0) atomicOr(flags, (int)GCCB_FLAG_EIG_NOCONV);
+  // NOCONV: the iteration limit reached with a residual the stopping rule would not accept even at stagnation (a
+  // residual below GCCB_CF_STAG that is still halving at the limit is better than what stagnation accepts)
+  if (!converged && !(prev_worst < GCCB_CF_STAG) && tid == 0) atomicOr(flags, (int)GCCB_FLAG_EIG_NOCONV);
   if (tid == 0) {
     dbg_iters[slot] = iter; dbg_res[slot] = prev_worst;
     for (int i = 0; i < 8; ++i) dbg_phase[(size_t)slot * 8 + i] = ph[i];
@@ -1110,14 +1114,20 @@ posenc_chfsi_cluster_kernel(const int32_t* __restrict__ worklist, const int32_t*
   float* X = dynsm;                                     // local slices: R x 49 each
   float* Y = dynsm + (size_t)C.R * LD;
   const int32_t* v_deg = sub_deg + (size_t)view * node_cap;
-  if (tid == 0) s_nheavy = 0;
-  __syncthreads();
-  for (int rl = tid; rl < nloc; rl += NT) {
-    int d = v_deg[noff + r_lo + rl];
-    if (d > GCCB_CL_HEAVY) {
-      int h = atomicAdd(&s_nheavy, 1);
-      if (h < GCCB_CL_MAXHEAVY) heavy[h] = rl;
+  // hub rows summed by the whole CTA: the first GCCB_CL_MAXHEAVY rows of degree > GCCB_CL_HEAVY in row order (a
+  // warp-ballot prefix), so which rows are listed -- and with it every row's summation order -- depends on the graph
+  // alone (the slab may hold more such rows than the list)
+  if (warp == 0) {
+    int cnt = 0;
+    for (int r0 = 0; r0 < nloc && cnt < GCCB_CL_MAXHEAVY; r0 += 32) {
+      const int rl = r0 + lane;
+      const bool h = rl < nloc && v_deg[noff + r_lo + rl] > GCCB_CL_HEAVY;
+      const unsigned m = __ballot_sync(0xffffffffu, h);
+      const int at = cnt + __popc(m & ((1u << lane) - 1u));
+      if (h && at < GCCB_CL_MAXHEAVY) heavy[at] = rl;
+      cnt += __popc(m);
     }
+    if (lane == 0) s_nheavy = cnt;
   }
   // every CTA needs all of dinv (neighbour weights): each writes its own rows, visible after the sync
   for (int rl = tid; rl < nloc; rl += NT) {
@@ -1310,7 +1320,7 @@ posenc_chfsi_cluster_kernel(const int32_t* __restrict__ worklist, const int32_t*
     GCCB_TICK(5);
   }
   if (C.rank == 0 && tid == 0) {
-    if (!converged) atomicOr(flags, (int)GCCB_FLAG_EIG_NOCONV);
+    if (!converged && !(prev_worst < GCCB_CF_STAG)) atomicOr(flags, (int)GCCB_FLAG_EIG_NOCONV);   // as above
     dbg_iters[slot] = iter; dbg_res[slot] = prev_worst;
     for (int i = 0; i < 8; ++i) dbg_phase[(size_t)slot * 8 + i] = ph[i];
   }

@@ -216,7 +216,7 @@ class BatchBuffers:
             if self.eig_noconv_events == 1:
                 import warnings
                 warnings.warn("gcc_b200: an ego-net eigensolve hit its iteration limit "
-                              "(residual above 2.5e-4); features kept as is")
+                              "with a residual above 2e-3; features kept as is")
             f &= ~_capi.FLAG_EIG_NOCONV
         if f:
             raise _lib.GccbError(where + "device flags: " + "; ".join(
