@@ -423,6 +423,8 @@ class NodeClassificationDataset(_EpochOrder):
         self.batch_size = B = int(min(batch_size, self.length))
         mb = self.graph.max_budget
         self.node_cap, self.edge_cap = walk_capacity(B, mb, node_cap, edge_cap, clip=320)
+        # a given capacity is a memory limit; at the default one, EmbedEngine re-runs a batch that overflows it
+        self.caps_given = node_cap is not None or edge_cap is not None
         self.buffers = BatchBuffers(B, self.node_cap, self.edge_cap, positional_embedding_size, mb, self.device)
         self.next_batch = 0
 

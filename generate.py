@@ -23,7 +23,9 @@ Node rows go through gcc_b200.embed.EmbedEngine (the data path of `--prefetch` b
 the graph.  `--nodes FILE` writes only the rows of the listed ids, in the file's order.  `--gpu 0 1 ...` splits the
 rows into one contiguous, batch-aligned shard per entry, each embedded by its own process on that device and written
 at its offsets in the shared file; the same id may repeat.  A row depends only on (run seed, node id), so the shards
-exchange nothing.
+exchange nothing.  A batch whose ego-nets overflow the default capacity (a run of hubs of a power-law graph) is re-run
+on buffers sized from its measured ego-nets; one line after the rows are saved says how many were, and the largest
+ego-net met.
 """
 import argparse
 import multiprocessing
@@ -117,6 +119,17 @@ def read_nodes(path):
     return ids.astype(np.int64)
 
 
+def replan_line(stats, n_batches):
+    """The line generate.py prints after the rows: batches re-planned of n_batches, from the shards' (count,
+    (vertices, edges) of the largest ego-net) results, and the largest ego-net met."""
+    count = sum(c for c, _ in stats)
+    if not count:
+        return "re-planned 0 of %d batches: every batch fit the default capacity" % n_batches
+    n, m = max(big for _, big in stats)
+    return ("re-planned %d of %d batches that overflowed the default capacity on buffers sized from their ego-nets; "
+            "largest ego-net met: %d vertices, %d edges" % (count, n_batches, n, m))
+
+
 def split_shards(n, batch_size, workers):
     """Rows 0..n-1 in batches of batch_size, split into `workers` contiguous runs of whole batches (the first
     n_batches mod workers runs get one batch more) -> one (lo, hi) per worker; workers beyond the batch count get
@@ -132,7 +145,8 @@ def split_shards(n, batch_size, workers):
 
 
 def _node_rows(load_path, graph, batch_size, prefetch, gpu, rows, out):
-    """Embed `rows` (a range of node ids or an int64 array of them) of `graph` on device `gpu` into `out`."""
+    """Embed `rows` (a range of node ids or an int64 array of them) of `graph` on device `gpu` into `out`.  Returns
+    (batches re-planned, (vertices, edges) of the largest ego-net they held)."""
     from gcc_b200.embed import EmbedEngine
     torch.cuda.set_device(gpu)
     dev = torch.device("cuda", gpu)
@@ -146,27 +160,31 @@ def _node_rows(load_path, graph, batch_size, prefetch, gpu, rows, out):
         dataset=graph, rw_hops=opt.rw_hops, subgraph_size=opt.subgraph_size, restart_prob=opt.restart_prob,
         positional_embedding_size=opt.positional_embedding_size, device=dev, seed=getattr(opt, "seed", 0),
         batch_size=batch_size)
-    EmbedEngine(nodes, encoder, prefetch=prefetch).run(rows, out)
+    eng = EmbedEngine(nodes, encoder, prefetch=prefetch)
+    eng.run(rows, out)
     torch.cuda.synchronize(dev)
+    return eng.replanned, eng.largest_egonet
 
 
-def _worker(load_path, dataset, graph_nodes, graph_edges, batch_size, prefetch, gpu, rows, out_file, lo, hi, errors):
-    """One shard in its own process: rows lo..hi-1 of the output file."""
+def _worker(load_path, dataset, graph_nodes, graph_edges, batch_size, prefetch, gpu, rows, out_file, lo, hi, conn):
+    """One shard in its own process: rows lo..hi-1 of the output file.  Sends _node_rows' result through conn, or
+    the traceback if it fails."""
     try:
         graph = resolve_graph(dataset, graph_nodes, graph_edges)
         out = np.lib.format.open_memmap(out_file, mode="r+")
-        _node_rows(load_path, graph, batch_size, prefetch, gpu, rows, out[lo:hi])
+        stats = _node_rows(load_path, graph, batch_size, prefetch, gpu, rows, out[lo:hi])
         out.flush()
     except BaseException:
-        errors.send(traceback.format_exc()[-WORKER_ERROR_CHARS:])
+        conn.send(traceback.format_exc()[-WORKER_ERROR_CHARS:])
         raise SystemExit(1)
+    conn.send(stats)
 
 
 def _run_shards(args_test, gpus, shards, rows_of, out_file, prefetch):
     """One process per non-empty shard; all of them joined.  If one fails, the others are terminated and its error
-    is raised."""
+    is raised.  Returns the shards' _node_rows results."""
     ctx = multiprocessing.get_context("spawn")
-    procs = []
+    procs, stats = [], []
     try:
         for i, (gpu, (lo, hi)) in enumerate(zip(gpus, shards)):
             if lo == hi:
@@ -188,6 +206,7 @@ def _run_shards(args_test, gpus, shards, rows_of, out_file, prefetch):
                         msg = recv.recv() if recv.poll() else "exit code %d" % p.exitcode
                         raise RuntimeError("generate.py: shard %d (gpu %d, rows %d..%d) failed:\n%s"
                                            % (i, gpu, lo, hi - 1, msg))
+                    stats.append(recv.recv())
     finally:
         for *_, p, recv in procs:
             if p.is_alive():
@@ -195,6 +214,7 @@ def _run_shards(args_test, gpus, shards, rows_of, out_file, prefetch):
         for *_, p, recv in procs:
             p.join()
             recv.close()
+    return stats
 
 
 def main(args_test):
@@ -246,19 +266,20 @@ def main(args_test):
     rows_of = (lambda lo, hi: range(lo, hi)) if ids is None else (lambda lo, hi: ids[lo:hi])
     out_file = out + ".npy"
     emb = np.lib.format.open_memmap(out_file, mode="w+", dtype=np.float32, shape=(n, opt.hidden_size))
+    B = min(args_test.batch_size, n_nodes)
     try:
         if len(gpus) == 1:
-            _node_rows(path, graph, args_test.batch_size, prefetch, gpus[0], rows_of(0, n), emb)
+            stats = [_node_rows(path, graph, args_test.batch_size, prefetch, gpus[0], rows_of(0, n), emb)]
         else:
             # shards aligned to the batches a one-GPU run makes, so every batch holds the same nodes
-            B = min(args_test.batch_size, n_nodes)
-            _run_shards(args_test, gpus, split_shards(n, B, len(gpus)), rows_of, out_file, prefetch)
+            stats = _run_shards(args_test, gpus, split_shards(n, B, len(gpus)), rows_of, out_file, prefetch)
         emb.flush()
     except BaseException:
         del emb
         os.remove(out_file)
         raise
     print("saved {} embeddings of dim {} to {}".format(n, opt.hidden_size, out_file))
+    print(replan_line(stats, -(-n // B)))
     return torch.from_numpy(np.asarray(emb))
 
 
