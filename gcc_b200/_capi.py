@@ -11,6 +11,7 @@ FLAG_NODE_OVERFLOW, FLAG_EDGE_OVERFLOW, FLAG_ZERO_DEGREE, FLAG_EIG_NOCONV, FLAG_
 FLAG_NAMES = {1: "node capacity overflow", 2: "edge capacity overflow",
               4: "walk reached a zero-degree vertex", 8: "eigensolver did not converge",
               16: "ego-net too large for the eigensolver"}
+FLAG_NONFINITE = 32                 # gccb_knn: an input row holds a NaN or an Inf
 
 p = C.c_void_p
 
@@ -155,6 +156,9 @@ _PROTOS = {
     "gccb_edgelist_begin": (C.c_int, [C.c_int32, p, C.c_size_t, p]),
     "gccb_edgelist_parse": (C.c_int, [p, C.c_int64, C.c_int32, p, C.c_int64, p, C.c_size_t, p]),
     "gccb_edgelist_finish": (C.c_int, [C.c_int32, p, p, C.c_size_t, p]),
+    "gccb_knn_workspace": (C.c_size_t, [C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32]),
+    "gccb_knn": (C.c_int, [p, C.c_int64, p, C.c_int64, C.c_int32, C.c_int32, p, C.c_int32, p, p, p, p, C.c_size_t,
+                           p]),
 }
 
 SYMBOLS = tuple(_PROTOS)

@@ -1,6 +1,8 @@
 """Frozen-embedding evaluators of the reference (gcc/tasks): node classification, graph classification and
 similarity search on the `.npy` rows generate.py writes.  They are scikit-learn fits on the host, as in the
-reference; at the datasets' sizes (a few thousand rows of 64) there is nothing for the GPU to do.
+reference; at the datasets' sizes (a few thousand rows of 64) there is nothing for the GPU to do.  Similarity
+search over the millions of rows generate.py writes for a large graph is `gcc_b200.tasks.knn`, an exact cosine top-k
+on the GPU.
 
     python -m gcc_b200.tasks.node_classification  --dataset usa_airport --model from_numpy --hidden-size 64 --emb-path <npy>
     python -m gcc_b200.tasks.graph_classification --dataset imdb-binary --model from_numpy_graph --hidden-size 64 --emb-path <npy>

@@ -43,6 +43,7 @@ typedef enum {
 #define GCCB_FLAG_ZERO_DEGREE 4     /* walk hit a vertex without successors (DGL: FATAL) */
 #define GCCB_FLAG_EIG_NOCONV 8      /* eigensolver hit its sweep/iteration limit        */
 #define GCCB_FLAG_EIG_TOOBIG 16     /* ego-net larger than the eigensolver supports     */
+#define GCCB_FLAG_NONFINITE 32      /* gccb_knn: an input row holds a NaN or an Inf     */
 
 int gccb_version(void);
 /* compute capability (major*10+minor) of the current device, or a negative status */
@@ -537,6 +538,31 @@ size_t gccb_prone_propagate_workspace(int64_t n, int32_t k);
 int gccb_prone_propagate(const int64_t* indptr, const int32_t* indices, const double* vals, int64_t n,
                          const double* a, int32_t k, double mu, const double* bessel, int32_t order,
                          void* workspace, size_t workspace_bytes, double* mm, gccb_stream_t stream);
+
+/* ---- structural similarity search: exact cosine top-k (csrc/knn.cu) ---------------------------------------
+ * The reference's evaluator (gcc/tasks/similarity_search.py) ranks with emb_2.dot(v).argsort() on the host; this is
+ * the same search at the sizes generate.py writes.  queries [nq][dim], cands [nc][dim]: fp32 rows, 1 <= dim <= 512.
+ *   normalisation (once per row): zero-pad to d4 = dim rounded up to 4; s = the sequential fmaf chain of x_j x_j over
+ *     j = 0 .. d4-1; x^_j = x_j / sqrtf(s), IEEE correctly rounded.  A row with s = 0 stays all zeros, so it scores 0
+ *     against everything (the reference divides by a zero norm and gets NaN).  A row holding a NaN or an Inf ORs
+ *     GCCB_FLAG_NONFINITE into *flags (caller clears); the results are then undefined.
+ *   score(q, c) = the sequential fmaf chain of q^_j c^_j over j = 0 .. d4-1, starting from +0.
+ *   result of query i: the first k candidates under (score descending, candidate index ascending), -0 == +0, never
+ *     exclude[i]: out_ids [nq][k] (int64) and out_scores [nq][k] (a score of -0 is written as +0), in that order.
+ * The order is strict and a score's bits depend on its two rows alone, so the output is a function of the inputs:
+ * it does not depend on `splits`, on how the queries are cut into calls, or on the device.
+ * exclude: [nq] device int64 or NULL; -1 (or any id outside 0..nc-1) excludes nothing.  1 <= k <= 128 and
+ * k <= nc - (exclude != NULL), else GCCB_ERR_BADARG; nc < 2^31.
+ * splits: candidate partitions of the score kernel (1 .. 128); 0 chooses them from (nq, nc) so that the grid fills
+ * the GPU.  cands == NULL reuses the normalised candidates an earlier call left at the start of the same workspace
+ * (same nc and dim), so a caller cutting its queries into several calls normalises the candidates once.
+ * Workspace, in bytes, 16-byte aligned, with ds = d4 rounded up to 32, S = the splits used, A(b) = b rounded up to 256:
+ *   A(nc * ds * 4)  normalised candidates  +  A(nq * ds * 4)  normalised queries  +  nq * S * k * 8  split lists.
+ * gccb_knn_workspace returns 0 for arguments gccb_knn refuses by shape.                                         */
+size_t gccb_knn_workspace(int64_t nq, int64_t nc, int32_t dim, int32_t k, int32_t splits);
+int gccb_knn(const float* queries, int64_t nq, const float* cands, int64_t nc, int32_t dim, int32_t k,
+             const int64_t* exclude, int32_t splits, int64_t* out_ids, float* out_scores, int32_t* flags, void* ws,
+             size_t ws_bytes, gccb_stream_t stream);
 
 #ifdef __cplusplus
 }
