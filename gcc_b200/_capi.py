@@ -12,6 +12,7 @@ FLAG_NAMES = {1: "node capacity overflow", 2: "edge capacity overflow",
               4: "walk reached a zero-degree vertex", 8: "eigensolver did not converge",
               16: "ego-net too large for the eigensolver"}
 FLAG_NONFINITE = 32                 # gccb_knn: an input row holds a NaN or an Inf
+FLAG_BAD_ROW = 64                   # gccb_seed_first_union: a row is not non-decreasing or leaves its graph
 
 p = C.c_void_p
 
@@ -96,6 +97,7 @@ _PROTOS = {
     "gccb_ns_batch": (C.c_int, [C.POINTER(Graph), p, p, p, C.c_int32, C.c_int32, C.POINTER(Batch), p, C.c_size_t,
                                 p]),
     "gccb_gather_graphs": (C.c_int, [C.POINTER(GraphSet), p, C.POINTER(Batch), p]),
+    "gccb_seed_first_union": (C.c_int, [C.POINTER(GraphSet), C.c_int64, C.c_int64, p, p, p, p, p]),
     "gccb_posenc_workspace": (C.c_size_t, [C.c_int32, C.c_int32]),
     "gccb_posenc": (C.c_int, [C.POINTER(Batch), C.c_int32, C.c_int32, p, p, p, C.c_size_t, p]),
     "gccb_gin_param_layout": (C.c_int, [C.POINTER(GinCfg), C.POINTER(GinLayout)]),

@@ -467,21 +467,126 @@ def seed_first_union(graphs):
     return seeds, items, indptr.astype(np.int64), indices, node_off, edge_off
 
 
+def first_bad_graph(indptr, indices, node_off):
+    """The first graph of a union CSR (host arrays) holding a row that is not non-decreasing or that names a vertex
+    outside the graph -- what gccb_seed_first_union reports as GCCB_FLAG_BAD_ROW -- or None."""
+    indptr, node_off = np.asarray(indptr, np.int64), np.asarray(node_off, np.int64)
+    indices = np.asarray(indices, np.int64)
+    row = np.repeat(np.arange(len(indptr) - 1), np.diff(indptr))
+    graph = np.searchsorted(node_off, row, side="right") - 1
+    bad = (indices < node_off[graph]) | (indices >= node_off[graph + 1])
+    bad[1:] |= (indices[1:] < indices[:-1]) & (row[1:] == row[:-1])
+    i = np.flatnonzero(bad)
+    return int(graph[i[0]]) if len(i) else None
+
+
+def sorted_rows(graph):
+    """graph with every row non-decreasing (a row's entries reordered, as seed_first orders them); graph itself when
+    its rows already are."""
+    indptr, indices = np.asarray(graph.indptr, np.int64), np.asarray(graph.indices)
+    if len(indices) < 2:
+        return graph
+    start = np.zeros(len(indices), bool)
+    start[indptr[:-1][np.diff(indptr) > 0]] = True
+    if not ((indices[1:] < indices[:-1]) & ~start[1:]).any():
+        return graph
+    row = np.repeat(np.arange(len(indptr) - 1), np.diff(indptr))
+    return synthetic.CSRGraph(indptr, indices[np.lexsort((indices, row))].astype(np.int32), graph.num_nodes,
+                              graph.name)
+
+
+def set_memory_error(n_nodes, n_edges, n_graphs, free):
+    """The message refusing a whole-graph set whose union CSR and its relabelled copy (int64 offsets, int32 ids, int64
+    graph offsets and seeds) do not fit in `free` bytes of device memory, or None when they fit."""
+    csr = 8 * (n_nodes + 1) + 4 * n_edges
+    need = 2 * csr + 8 * (3 * n_graphs + 2)
+    if need <= free:
+        return None
+    return ("a set of %d graphs (%d vertices, %d edge entries) needs %.2f GB of device memory for its union CSR and "
+            "its relabelled copy (%.2f GB each), %.2f GB are free; sets that do not fit are not supported"
+            % (n_graphs, n_nodes, n_edges, need / 1e9, csr / 1e9, free / 1e9))
+
+
 class DeviceGraphSet:
-    """Whole graphs relabelled seed first (seed_first_union; seeds, items, node offsets, sizes kept on the host), their
-    union CSR on the device as a gccb_graph_set_t, and the positional-feature cache (rows per vertex, eigenvalues per
-    graph).  Datasets and their fold views share one by reference."""
+    """Whole graphs relabelled seed first on the device (gccb_seed_first_union: seeds, node offsets and sizes kept on
+    the host), their union CSR on the device as a gccb_graph_set_t, and the positional-feature cache (rows per vertex,
+    eigenvalues per graph).  Datasets and their fold views share one by reference.  DeviceGraphSet(graphs) takes a list
+    of CSRGraphs; from_union takes the (union, sizes) load_graphs returns, and makes no per-graph host arrays.  The
+    whole union is uploaded, then relabelled into a copy; the input is freed once the copy is made."""
 
     def __init__(self, graphs, device):
-        self.device = torch.device(device)
-        self.seeds, self.items, indptr, indices, self.node_off_host, edge_off = seed_first_union(graphs)
-        self.sizes, self.nnz = np.diff(self.node_off_host), np.diff(edge_off)
-        to = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a)).to(device=self.device, dtype=dt)
-        self.indptr, self.indices = to(indptr, torch.int64), to(indices, torch.int32)
-        self.node_off, self.edge_off = to(self.node_off_host, torch.int64), to(edge_off, torch.int64)
+        graphs = list(graphs)
+        # seed_first_union sorts each relabelled row; the device relabel keeps rows non-decreasing, so it is given
+        # non-decreasing rows
+        union = sorted_rows(synthetic.disjoint_union(graphs))
+        self._build(union.indptr, union.indices, [g.num_nodes for g in graphs], device, "the graph list")
+
+    @classmethod
+    def from_union(cls, union, sizes, device, name="the union"):
+        """The set of graphs `sizes` (vertex counts, in order) of the union CSRGraph `union`, whose rows must be
+        non-decreasing and stay inside their graph (GccbError names the first graph that breaks this)."""
+        self = cls.__new__(cls)
+        self._build(union.indptr, union.indices, sizes, device, name)
+        return self
+
+    def _build(self, indptr, indices, sizes, device, name):
+        self.device = dev = torch.device(device)
+        sizes = np.asarray(sizes, dtype=np.int64).reshape(-1)
+        node_off = np.zeros(len(sizes) + 1, dtype=np.int64)
+        np.cumsum(sizes, out=node_off[1:])
+        indptr = np.ascontiguousarray(indptr, dtype=np.int64)
+        G, V = len(sizes), int(node_off[-1])
+        if G == 0 or sizes.min() < 0 or len(indptr) != V + 1:
+            raise ValueError("%s: graph sizes (%d graphs, %d vertices) do not match a CSR of %d rows"
+                             % (name, G, V, len(indptr) - 1))
+        E = int(indptr[-1])
+        if V > 2 ** 31:
+            raise _lib.GccbError("%s: %d vertices; union vertex ids must fit int32" % (name, V))
+        _lib.require_device()
+        with torch.cuda.device(dev):
+            free = torch.cuda.mem_get_info()[0] + torch.cuda.memory_reserved() - torch.cuda.memory_allocated()
+        msg = set_memory_error(V, E, G, free)
+        if msg:
+            raise _lib.GccbError("%s: %s" % (name, msg))
+        edge_off = indptr[node_off]
+        to = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a)).to(device=dev, dtype=dt)
+        src_ptr, src_idx = to(indptr, torch.int64), to(indices, torch.int32)
+        self.node_off, self.edge_off = to(node_off, torch.int64), to(edge_off, torch.int64)
+        src = _capi.GraphSet(src_ptr.data_ptr(), src_idx.data_ptr(), self.node_off.data_ptr(),
+                             self.edge_off.data_ptr(), G)
+        self.indptr = torch.empty(V + 1, dtype=torch.int64, device=dev)
+        self.indices = torch.empty(E, dtype=torch.int32, device=dev)
+        seeds = torch.empty(G, dtype=torch.int64, device=dev)
+        flags = torch.zeros(1, dtype=torch.int32, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(_lib.get().gccb_seed_first_union(C.byref(src), V, E, _lib.dptr(seeds), _lib.dptr(self.indptr),
+                                                        _lib.dptr(self.indices), _lib.dptr(flags), _lib.stream_ptr()),
+                       "gccb_seed_first_union")
+        if int(flags.item()):
+            g = first_bad_graph(indptr, np.asarray(indices), node_off)
+            raise _lib.GccbError("%s: graph %d has a row that is not non-decreasing or names a vertex outside the "
+                                 "graph" % (name, g))
+        del src_ptr, src_idx
+        self.seeds = seeds.cpu().numpy()
+        self.node_off_host = node_off
+        self.sizes, self.nnz = sizes, np.diff(edge_off)
         self.c = _capi.GraphSet(self.indptr.data_ptr(), self.indices.data_ptr(), self.node_off.data_ptr(),
-                                self.edge_off.data_ptr(), len(graphs))
+                                self.edge_off.data_ptr(), G)
         self.features = self.eigvals = None
+        self._items = None
+
+    def __len__(self):
+        return len(self.sizes)
+
+    @property
+    def items(self):
+        """[(indptr int64, indices int32)] per relabelled graph in local ids, as seed_first_union lists them: copied
+        from the device union on first use."""
+        if self._items is None:
+            ip, ix, no = self.indptr.cpu().numpy(), self.indices.cpu().numpy(), self.node_off_host
+            self._items = [(ip[a:b + 1] - ip[a], (ix[ip[a]:ip[b]] - a).astype(np.int32))
+                           for a, b in zip(no[:-1], no[1:])]
+        return self._items
 
     def buffers(self, B, pos_dim):
         """BatchBuffers that hold any B graphs of the set: the capacity of the B largest, plus 8, and no sampler
@@ -499,7 +604,7 @@ class DeviceGraphSet:
         computed on first use, in batches of B consecutive ids, whose rows are the union's rows in order.  The
         eigensolver is deterministic, so these are what gccb_posenc computes for a graph in any batch."""
         if self.features is None:
-            no, n = self.node_off_host, len(self.items)
+            no, n = self.node_off_host, len(self.sizes)
             cache = torch.empty(int(no[-1]), pos_dim, dtype=torch.float32, device=self.device)
             eigvals = torch.empty(n, pos_dim, dtype=torch.float32, device=self.device)
             full = self.buffers(B, pos_dim)
@@ -525,11 +630,74 @@ class DeviceGraphSet:
         torch.index_select(self.eigvals, 0, ids, out=buf.eigvals[:buf.B])
 
 
+INT32_MAX = 2 ** 31 - 1     # the batch layout's offsets are int32
+
+
+def whole_graph_plan(sizes, nnz, ids, B):
+    """(node_cap, edge_cap) of buffers that hold every batch of whole graphs `ids` (graph ids, in order; batches are
+    every B of them): the largest batch's vertex and edge-entry totals, plus 8.  GccbError names a batch that does not
+    fit the int32 batch layout, and its largest graph."""
+    ids = np.asarray(ids, dtype=np.int64)
+    if not len(ids):
+        return 8, 8
+    starts = np.arange(0, len(ids), B)
+    n = np.add.reduceat(np.asarray(sizes, np.int64)[ids], starts)
+    m = np.add.reduceat(np.asarray(nnz, np.int64)[ids], starts)
+    node_cap, edge_cap = int(n.max()) + 8, int(m.max()) + 8
+    if max(node_cap, edge_cap) > INT32_MAX:
+        t = int(np.argmax(np.maximum(n, m)))
+        chunk = ids[t * B:(t + 1) * B]
+        big = int(chunk[np.argmax(np.asarray(nnz, np.int64)[chunk])])
+        raise _lib.GccbError("batch of rows %d..%d (graph ids %d..%d): %d vertices and %d edge entries exceed the "
+                             "int32 batch layout; its largest graph, %d, has %d vertices and %d edge entries"
+                             % (t * B, t * B + len(chunk) - 1, chunk[0], chunk[-1], n[t], m[t], big, sizes[big],
+                                nnz[big]))
+    return node_cap, edge_cap
+
+
+class WholeGraphDataset:
+    """generate.py's whole-graph rows (graph_dataset.py:311-340 with entire_graph=True): item i is graph i of a
+    corpus, relabelled seed first on the device (DeviceGraphSet), and its row is the encoding of the whole graph.
+    `dataset` is a list of CSRGraphs, or the (union CSRGraph, sizes) pair load_graphs returns for a .bin or .npz
+    corpus.  EmbedEngine takes it as its dataset: its ring buffers are sized exactly from the batches it runs (plan),
+    and a batch's data path (prepare) is the gather of its graphs, view 1 marked absent, and the positional features
+    of view 0."""
+
+    whole_graphs = True
+
+    def __init__(self, dataset, positional_embedding_size=32, device="cuda", batch_size=256, name="the corpus"):
+        assert positional_embedding_size > 1
+        self.device = torch.device(device)
+        if isinstance(dataset, tuple) and len(dataset) == 2 and isinstance(dataset[0], synthetic.CSRGraph):
+            self.graph_set = DeviceGraphSet.from_union(dataset[0], dataset[1], self.device, name)
+        else:
+            self.graph_set = DeviceGraphSet(dataset, self.device)
+        self.positional_embedding_size = positional_embedding_size
+        self.length = self.total = len(self.graph_set)
+        self.batch_size = int(min(batch_size, self.total))
+
+    def plan(self, ids):
+        """(node_cap, edge_cap) for the batches of the graph ids `ids` (whole_graph_plan)."""
+        gs = self.graph_set
+        return whole_graph_plan(gs.sizes, gs.nnz, ids, self.batch_size)
+
+    def buffers(self, node_cap, edge_cap):
+        return BatchBuffers(self.batch_size, node_cap, edge_cap, self.positional_embedding_size, None, self.device)
+
+    def prepare(self, buf, ids):
+        """View 0 of buf = the whole graphs `ids` (device int64 [buf.B]) with their positional features; view 1 marked
+        absent, so the eigensolver solves view 0 alone.  No host sync."""
+        self.graph_set.gather(ids, buf)
+        buf.mark_absent(1)
+        buf.posenc()
+        return buf
+
+
 class GraphClassificationDataset(_EpochOrder):
     """graph_dataset.py:311-340 (entire_graph=True) for pretraining: item idx is GRAPH idx, and q and k are
     both the whole graph with its seed on the first maximum out-degree vertex.  The reference also walks an
     RWR trace per view and then discards it; nothing is walked here.  Each graph is relabelled seed first
-    once, here (labeled.seed_first), and the set lives on the device as one union CSR; a batch is
+    once, on the device (DeviceGraphSet), and the set lives there as one union CSR; a batch is
     gccb_gather_graphs of the epoch's next graph ids.  Positional features come from a deterministic
     eigensolver, so the two views' features are identical (the reference starts ARPACK from a random vector
     per view).  `dataset` is a name of downstream.GRAPH_DSETS (TU files under ./data), a list of CSRGraphs or
@@ -555,11 +723,16 @@ class GraphClassificationDataset(_EpochOrder):
         self.device = torch.device(device)
         _lib.require_device()
         self.graph_set = DeviceGraphSet(graphs, self.device)
-        self.seeds, self.items = self.graph_set.seeds, self.graph_set.items      # each item's seed and graph
+        self.seeds = self.graph_set.seeds                                    # each item's seed
         self.batch_size = B = int(min(batch_size, self.total))
         self.buffers = self.graph_set.buffers(B, positional_embedding_size)
         self.node_cap, self.edge_cap = self.buffers.node_cap, self.buffers.edge_cap
         self.next_batch = 0
+
+    @property
+    def items(self):
+        """Each item's relabelled graph (DeviceGraphSet.items)."""
+        return self.graph_set.items
 
     def sample_batch(self, first_sample=None, seeds=None, buffers=None, posenc=True):
         """Batch number first_sample // B of the epoch order: graphs a .. a+b-1 in both views, on the device with

@@ -9,7 +9,7 @@ gcc/datasets/data_util.py:35-113,227-236, train.py:516-545).
       (entire_graph=True, seed = argmax out-degree,        (data_util.py:227-236), the seed one-hot sits on the
       cached in self.dict at construction :355)            max-degree node.  The device batch layout marks row 0 of
                                                            each graph as the seed, so each graph is relabelled once
-                                                           (seed first) on the host; GIN, sum pooling and the
+                                                           (seed first, on the device); GIN, sum pooling and the
                                                            eigenvector features are permutation-equivariant.
   labeled_batcher() data_util.py:35-41                   batches(): (BatchedSubgraphs, LongTensor labels)
   Edgelist data_util.py:61-113                           Edgelist (same file formats, own parser)
@@ -342,7 +342,7 @@ class GraphClassificationDatasetLabeled(_LabeledBase):
         # the reference's self.dict (:355): every item is prepared once.  seed = argmax degree (:361, first
         # maximum), moved to row 0; the relabelled items form one union CSR on the device
         self.graph_set = DeviceGraphSet(graphs, self.device)
-        self.seeds, self.items = self.graph_set.seeds, self.graph_set.items      # each item's seed and graph
+        self.seeds = self.graph_set.seeds                                    # each item's seed
         self.batch_size = int(min(batch_size, self.length))
         self._bufs = {}
         self.labels_dev = torch.from_numpy(self.labels).to(self.device)      # FinetuneEngine's label table
@@ -365,6 +365,11 @@ class GraphClassificationDatasetLabeled(_LabeledBase):
             return read_tu_dataset("data", _TU_NAMES[dataset])
         raise NotImplementedError("graph classification dataset %r: pass (graphs, labels), an .npz or one of %s"
                                   % (dataset, GRAPH_CLASSIFICATION_DSETS))
+
+    @property
+    def items(self):
+        """Each item's relabelled graph (DeviceGraphSet.items)."""
+        return self.graph_set.items
 
     def _new_buffers(self, B):
         return self.graph_set.buffers(B, self.positional_embedding_size)

@@ -11,6 +11,12 @@ The host waits on one event per batch, when it takes the batch's rows out of the
 is reused.  The batch's device flag word travels with its rows into pinned memory, so reading it costs no further
 sync.  Host memory is the staging ring, (S+1) x B x hidden floats, whatever the number of nodes.
 
+A WholeGraphDataset (one row per graph of a corpus, DESIGN §5f) runs through the same ring.  The dataset decides a
+batch's data path: the gather of its whole graphs, view 1 marked absent, and the positional features of view 0; the
+encoder runs view 0 alone, since q and k are the same graph and (x + x) / 2 == x.  The host knows every graph's
+size, so run() sizes the ring's buffers exactly, from the largest batch it will run; a whole-graph batch never
+overflows and is never re-run.
+
 A batch whose ego-nets overflow a dataset of the default capacity is re-run after the ring has drained, on spill
 buffers of the engine's own (DESIGN §5e): sampled again with the same sample ids, so with the same walks, its
 counters read (one host sync), and its ego-nets cut into consecutive groups that fit (spill_groups).
@@ -57,13 +63,16 @@ def spill_groups(sizes, exact, node_cap, edge_cap):
 
 class EmbedEngine:
     def __init__(self, dataset, model, prefetch=4):
-        """dataset: a NodeClassificationDataset; model: a GraphEncoder on the dataset's device.  prefetch: S, the
+        """dataset: a NodeClassificationDataset or a WholeGraphDataset; model: a GraphEncoder on the dataset's
+        device.  prefetch: S, the
         batches whose data path runs ahead of the encoder; 0 runs every stage of a batch on the caller's stream and
         waits for its rows before the next batch starts (the serial loop)."""
         _lib.require_device()
         self.ds, self.model = dataset, model
+        self.whole = getattr(dataset, "whole_graphs", False)
+        self.item = "graph" if self.whole else "node"
         # a caller who gave the dataset a capacity has set a memory limit: an overflowing batch raises
-        self.replan = not dataset.caps_given
+        self.replan = not self.whole and not dataset.caps_given
         self.dev = model.flat_params.device
         self.B, self.H = B, H = dataset.batch_size, model.cfg.hidden
         self.prefetch = S = int(prefetch)
@@ -71,11 +80,15 @@ class EmbedEngine:
             raise ValueError("prefetch must be >= 0, got %d" % S)
         self.depth = S + 1
         ds = dataset
-        self.bufs = [ds.buffers] + [BatchBuffers(B, ds.node_cap, ds.edge_cap, ds.buffers.pos_dim,
-                                                 ds.buffers.max_budget, self.dev) for _ in range(S)]
+        if self.whole:
+            self.bufs = self.acts = None               # sized by run() from the batches it runs (_size_ring)
+            self.node_cap = self.edge_cap = 0
+        else:
+            self.bufs = [ds.buffers] + [BatchBuffers(B, ds.node_cap, ds.edge_cap, ds.buffers.pos_dim,
+                                                     ds.buffers.max_budget, self.dev) for _ in range(S)]
+            # the encoder stream runs batches one after another, so one set of activations serves them all
+            self.acts = torch.empty(model.acts_bytes(B, ds.node_cap), dtype=torch.uint8, device=self.dev)
         f32 = dict(dtype=torch.float32, device=self.dev)
-        # the encoder stream runs batches one after another, so one set of activations and features serves them all
-        self.acts = torch.empty(model.acts_bytes(B, ds.node_cap), dtype=torch.uint8, device=self.dev)
         self.feat_q, self.feat_k, self.avg = (torch.empty(B, H, **f32) for _ in range(3))
         # the host side: one pinned slot of rows and one flag word per ring slot
         self.stage = torch.empty(self.depth, B, H, dtype=torch.float32).pin_memory()
@@ -95,19 +108,22 @@ class EmbedEngine:
         """Rows (f(q) + f(k)) / 2 of `nodes` (a range of node ids, or a 1-D int64 sequence of them) written to out[i]
         for the i-th id: a float32 array-like [len(nodes), hidden] such as a numpy memmap, or a new array if None.
         A batch whose ego-nets overflow the dataset's default capacity is re-run after the others on buffers sized from
-        them (_replan); when the caller gave the dataset its capacity, GccbError is raised naming the batch's nodes."""
-        n_nodes = self.ds.graph.num_nodes
+        them (_replan); when the caller gave the dataset its capacity, GccbError is raised naming the batch's nodes.
+        On a WholeGraphDataset, `nodes` are graph ids and a row is f(graph)."""
+        n_nodes = self.ds.total if self.whole else self.ds.graph.num_nodes
         if isinstance(nodes, range):
             if nodes.step != 1 or (len(nodes) and not 0 <= nodes.start < nodes.stop <= n_nodes):
-                raise ValueError("node range %r is not a contiguous part of 0..%d" % (nodes, n_nodes - 1))
+                raise ValueError("%s range %r is not a contiguous part of 0..%d" % (self.item, nodes, n_nodes - 1))
             self._first, self._ids = nodes.start, None
         else:
             ids = np.ascontiguousarray(np.asarray(nodes, dtype=np.int64).reshape(-1))
             if ids.size and (ids.min() < 0 or ids.max() >= n_nodes):
-                raise ValueError("node ids must lie in 0..%d" % (n_nodes - 1))
+                raise ValueError("%s ids must lie in 0..%d" % (self.item, n_nodes - 1))
             self._ids_host = ids
             self._ids = torch.from_numpy(ids).pin_memory().to(self.dev, non_blocking=True)
         self.n = n = len(nodes)
+        if self.whole:
+            self._size_ring(np.arange(nodes.start, nodes.stop) if self._ids is None else self._ids_host)
         if out is None:
             out = np.empty((n, self.H), dtype=np.float32)
         if tuple(out.shape) != (n, self.H):
@@ -145,6 +161,19 @@ class EmbedEngine:
         return out
 
     # -------------------------------------------------------------------------------------------
+    def _size_ring(self, ids):
+        """Whole graphs: the ring's buffers and activations sized for the largest batch of `ids` (the dataset's plan),
+        reallocated when the plan changes."""
+        caps = self.ds.plan(ids)
+        if self.bufs is not None and caps == (self.node_cap, self.edge_cap):
+            return
+        if self.bufs is not None and self.prefetch:
+            torch.cuda.current_stream(self.dev).wait_stream(self.enc_stream)   # an earlier run's work on them
+        self.bufs = self.acts = None                   # freed before the new ones are allocated
+        self.node_cap, self.edge_cap = caps
+        self.bufs = [self.ds.buffers(*caps) for _ in range(self.depth)]
+        self.acts = torch.empty(self.model.acts_bytes(self.B, caps[0]), dtype=torch.uint8, device=self.dev)
+
     def _rows(self, j):
         a = j * self.B
         return a, min(self.B, self.n - a)
@@ -161,8 +190,11 @@ class EmbedEngine:
                 torch.arange(self._first + a, self._first + a + b, device=self.dev, out=buf.seeds)
             else:
                 buf.seeds.copy_(self._ids[a:a + b], non_blocking=True)
-            sample_pairs(self.ds, buf, None, buf.seeds, sample_ids=buf.seeds)     # sample id of node v is v
-            buf.posenc()
+            if self.whole:
+                self.ds.prepare(buf, buf.seeds)
+            else:
+                sample_pairs(self.ds, buf, None, buf.seeds, sample_ids=buf.seeds)     # sample id of node v is v
+                buf.posenc()
             self.ready[slot].record()
 
     def _encode(self, t):
@@ -173,18 +205,26 @@ class EmbedEngine:
         st = self.enc_stream if self.prefetch else torch.cuda.current_stream(self.dev)
         st.wait_event(self.ready[slot])
         with torch.cuda.stream(st):
-            avg = self._forward_mean(buf, self.acts, self.feat_q[:b], self.feat_k[:b], self.avg[:b])
+            if self.whole:                             # q = k = the graph: (f + f) / 2 = f, bit for bit
+                avg = self._forward_view(buf, 0, self.acts, self.feat_q[:b])
+            else:
+                avg = self._forward_mean(buf, self.acts, self.feat_q[:b], self.feat_k[:b], self.avg[:b])
             self.flag_stage[slot:slot + 1].copy_(buf.flags, non_blocking=True)
             buf.flags.zero_()
             self.consumed[slot].record()
             self.stage[slot, :b].copy_(avg, non_blocking=True)
             self.staged[slot].record()
 
+    def _forward_view(self, buf, v, acts, feat):
+        """View v of the batch in buf through the encoder in eval mode, into feat."""
+        self.model._run_forward(BatchedSubgraphs(buf, v), False, step=0, dropout=False, acts=acts,
+                                feat=feat, all_outputs=False, bn_train=False)
+        return feat
+
     def _forward_mean(self, buf, acts, fq, fk, avg):
         """Both views of the batch in buf through the encoder in eval mode, then avg = (fq + fk) / 2."""
         for v, feat in ((0, fq), (1, fk)):
-            self.model._run_forward(BatchedSubgraphs(buf, v), False, step=0, dropout=False, acts=acts,
-                                    feat=feat, all_outputs=False, bn_train=False)
+            self._forward_view(buf, v, acts, feat)
         torch.add(fq, fk, out=avg)
         avg.mul_(0.5)                                  # = torch.stack([fq, fk]).mean(0), bit for bit
         return avg
@@ -192,9 +232,9 @@ class EmbedEngine:
     def _where(self, t):
         a, b = self._rows(t)
         if self._ids is None:
-            return "batch of nodes %d..%d: " % (self._first + a, self._first + a + b - 1)
-        return "batch of rows %d..%d (node ids %d..%d in the given order): " % (
-            a, a + b - 1, self._ids_host[a], self._ids_host[a + b - 1])
+            return "batch of %ss %d..%d: " % (self.item, self._first + a, self._first + a + b - 1)
+        return "batch of rows %d..%d (%s ids %d..%d in the given order): " % (
+            a, a + b - 1, self.item, self._ids_host[a], self._ids_host[a + b - 1])
 
     def _drain(self, t):
         """Host: wait for batch t's slot, check its flags, copy its rows to the output, or record the batch for a

@@ -15,17 +15,23 @@ the same.
     multigraph of the reference's _create_dgl_graph, parallel edges kept, one row per node;
   - .bin corpora (datasets/dgl_bin.py, as train.py and x2dgl read and write them): one row per vertex of the union
     of the file's graphs, in file order (the ids load_graphs assigns);
-  - graph datasets (the five TU sets from data/<NAME>): q and k are both the whole graph with the seed on its first
-    maximum-degree vertex (entire_graph=True), so the row of a graph is the encoding of that whole graph.
+  - graph datasets (the five TU sets from data/<NAME>, or a path to any TU directory NAME holding NAME_A.txt,
+    NAME_graph_indicator.txt, ...): q and k are both the whole graph with the seed on its first maximum-degree vertex
+    (entire_graph=True), so the row of a graph is the encoding of that whole graph; one row per graph, in the file's
+    order.  A TU directory's rows go to `<model_folder>/<NAME>.npy`;
+  - `--whole-graphs` on a .bin or .npz corpus with graph_sizes: one whole-graph row per graph of the file, in file
+    order, saved as `<model_folder>/<stem>.graphs.npy` beside the vertex rows `<stem>.npy`.
 
-Node rows go through gcc_b200.embed.EmbedEngine (the data path of `--prefetch` batches runs ahead of the encoder;
+Node and whole-graph rows go through gcc_b200.embed.EmbedEngine (the data path of `--prefetch` batches runs ahead of the encoder;
 `--prefetch 0` is the serial loop) straight into the .npy file through a memmap, so host memory does not grow with
-the graph.  `--nodes FILE` writes only the rows of the listed ids, in the file's order.  `--gpu 0 1 ...` splits the
+the graph.  `--nodes FILE` writes only the rows of the listed ids (node ids, or graph ids for whole graphs), in the file's
+order.  `--gpu 0 1 ...` splits the
 rows into one contiguous, batch-aligned shard per entry, each embedded by its own process on that device and written
 at its offsets in the shared file; the same id may repeat.  A row depends only on (run seed, node id), so the shards
 exchange nothing.  A batch whose ego-nets overflow the default capacity (a run of hubs of a power-law graph) is re-run
 on buffers sized from its measured ego-nets; one line after the rows are saved says how many were, and the largest
-ego-net met.
+ego-net met.  Whole graphs are relabelled seed first on the device (gccb_seed_first_union), and the ring's buffers are
+sized from the largest batch that runs, so no whole-graph batch overflows; each process uploads the whole union.
 """
 import argparse
 import multiprocessing
@@ -37,8 +43,8 @@ import numpy as np
 import torch
 
 from gcc_b200.datasets import downstream, synthetic
-from gcc_b200.datasets.graph_dataset import NodeClassificationDataset, load_graphs
-from gcc_b200.datasets.labeled import GraphClassificationDatasetLabeled
+from gcc_b200.datasets.graph_dataset import NodeClassificationDataset, WholeGraphDataset, load_graphs
+from gcc_b200.datasets.labeled import read_tu_dataset
 from gcc_b200.models import GraphEncoder
 
 # checkpoint["opt"] attribute -> GraphEncoder keyword (train.py:601-620 builds the model from these)
@@ -66,17 +72,41 @@ def test_moco(train_loader, model, opt):
     return torch.cat(chunks)
 
 
-def test_graphs(dataset, model, opt):
-    """Embedding of every whole graph (graph datasets): q = k = the graph, so (f(q) + f(k)) / 2 = f(graph)."""
-    model.eval()
-    chunks = []
-    with torch.no_grad():
-        for graph, _ in dataset.batches():
-            feat = model(graph)
-            if feat.shape != (graph.batch_size, opt.hidden_size):
-                raise RuntimeError("encoder returned %s" % (tuple(feat.shape),))
-            chunks.append(feat.cpu())
-    return torch.cat(chunks)
+def is_tu_dir(path):
+    """A TU directory NAME holding NAME_A.txt (and NAME_graph_indicator.txt, ...)."""
+    name = os.path.basename(os.path.normpath(path))
+    return os.path.isdir(path) and os.path.isfile(os.path.join(path, name + "_A.txt"))
+
+
+def whole_graph_source(dataset):
+    """A TU name, a TU directory, or None when `dataset` names no graph set (a .bin / .npz corpus embeds whole
+    graphs only with --whole-graphs)."""
+    if dataset in downstream.GRAPH_DSETS:
+        return "tu-name"
+    if is_tu_dir(dataset):
+        return "tu-dir"
+    return None
+
+
+def resolve_whole_graphs(dataset):
+    """The graphs `dataset` embeds whole: a list of CSRGraphs (TU sets, read as multigraphs, as the named sets are)
+    or the (union, sizes) load_graphs returns for a .bin / .npz corpus."""
+    kind = whole_graph_source(dataset)
+    if kind == "tu-name":
+        return downstream.graph_dataset_graphs(dataset)[0]
+    if kind == "tu-dir":
+        path = os.path.normpath(dataset)
+        return read_tu_dataset(os.path.dirname(path), os.path.basename(path), multigraph=True)[0]
+    return load_graphs(dataset)
+
+
+def output_stem(dataset, whole_graphs):
+    """The output file's name without .npy: the dataset name, a TU directory's NAME, or a corpus file's stem (with
+    .graphs for its whole-graph rows, so they never overwrite its vertex rows)."""
+    stem = os.path.basename(os.path.normpath(dataset))
+    if stem.endswith(".npz") or stem.endswith(".bin"):
+        stem = stem[:-4] + (".graphs" if whole_graphs else "")
+    return stem
 
 
 def resolve_graph(name, nodes, edges):
@@ -144,9 +174,10 @@ def split_shards(n, batch_size, workers):
     return out
 
 
-def _node_rows(load_path, graph, batch_size, prefetch, gpu, rows, out):
+def _node_rows(load_path, graph, batch_size, prefetch, gpu, rows, out, whole=False):
     """Embed `rows` (a range of node ids or an int64 array of them) of `graph` on device `gpu` into `out`.  Returns
-    (batches re-planned, (vertices, edges) of the largest ego-net they held)."""
+    (batches re-planned, (vertices, edges) of the largest ego-net they held).  whole: `graph` is what
+    resolve_whole_graphs returns, `rows` are graph ids, and the result is (0, (node_cap, edge_cap) of the ring)."""
     from gcc_b200.embed import EmbedEngine
     torch.cuda.set_device(gpu)
     dev = torch.device("cuda", gpu)
@@ -156,23 +187,30 @@ def _node_rows(load_path, graph, batch_size, prefetch, gpu, rows, out):
     encoder.load_state_dict(ckpt["model"])
     encoder = encoder.to(dev).eval()
     del ckpt
-    nodes = NodeClassificationDataset(
-        dataset=graph, rw_hops=opt.rw_hops, subgraph_size=opt.subgraph_size, restart_prob=opt.restart_prob,
-        positional_embedding_size=opt.positional_embedding_size, device=dev, seed=getattr(opt, "seed", 0),
-        batch_size=batch_size)
-    eng = EmbedEngine(nodes, encoder, prefetch=prefetch)
+    if whole:
+        items = WholeGraphDataset(graph, positional_embedding_size=opt.positional_embedding_size, device=dev,
+                                  batch_size=batch_size)
+    else:
+        items = NodeClassificationDataset(
+            dataset=graph, rw_hops=opt.rw_hops, subgraph_size=opt.subgraph_size, restart_prob=opt.restart_prob,
+            positional_embedding_size=opt.positional_embedding_size, device=dev, seed=getattr(opt, "seed", 0),
+            batch_size=batch_size)
+    eng = EmbedEngine(items, encoder, prefetch=prefetch)
     eng.run(rows, out)
     torch.cuda.synchronize(dev)
+    if whole:
+        return 0, (eng.node_cap, eng.edge_cap)
     return eng.replanned, eng.largest_egonet
 
 
-def _worker(load_path, dataset, graph_nodes, graph_edges, batch_size, prefetch, gpu, rows, out_file, lo, hi, conn):
+def _worker(load_path, dataset, graph_nodes, graph_edges, batch_size, prefetch, gpu, rows, out_file, lo, hi, conn,
+            whole=False):
     """One shard in its own process: rows lo..hi-1 of the output file.  Sends _node_rows' result through conn, or
     the traceback if it fails."""
     try:
-        graph = resolve_graph(dataset, graph_nodes, graph_edges)
+        graph = resolve_whole_graphs(dataset) if whole else resolve_graph(dataset, graph_nodes, graph_edges)
         out = np.lib.format.open_memmap(out_file, mode="r+")
-        stats = _node_rows(load_path, graph, batch_size, prefetch, gpu, rows, out[lo:hi])
+        stats = _node_rows(load_path, graph, batch_size, prefetch, gpu, rows, out[lo:hi], whole)
         out.flush()
     except BaseException:
         conn.send(traceback.format_exc()[-WORKER_ERROR_CHARS:])
@@ -180,7 +218,7 @@ def _worker(load_path, dataset, graph_nodes, graph_edges, batch_size, prefetch, 
     conn.send(stats)
 
 
-def _run_shards(args_test, gpus, shards, rows_of, out_file, prefetch):
+def _run_shards(args_test, gpus, shards, rows_of, out_file, prefetch, whole=False):
     """One process per non-empty shard; all of them joined.  If one fails, the others are terminated and its error
     is raised.  Returns the shards' _node_rows results."""
     ctx = multiprocessing.get_context("spawn")
@@ -192,7 +230,8 @@ def _run_shards(args_test, gpus, shards, rows_of, out_file, prefetch):
             recv, send = ctx.Pipe(duplex=False)
             p = ctx.Process(target=_worker, name="generate-shard-%d" % i,
                             args=(args_test.load_path, args_test.dataset, args_test.graph_nodes, args_test.graph_edges,
-                                  args_test.batch_size, prefetch, gpu, rows_of(lo, hi), out_file, lo, hi, send))
+                                  args_test.batch_size, prefetch, gpu, rows_of(lo, hi), out_file, lo, hi, send,
+                                  whole))
             p.start()
             send.close()
             procs.append((i, gpu, lo, hi, p, recv))
@@ -230,56 +269,51 @@ def main(args_test):
     gpus = parse_gpus(getattr(args_test, "gpu", None))
     prefetch = getattr(args_test, "prefetch", 4)
     nodes_file = getattr(args_test, "nodes", None)
-    stem = os.path.basename(args_test.dataset)
-    stem = stem[:-4] if stem.endswith(".npz") or stem.endswith(".bin") else stem
-    out = os.path.join(getattr(opt, "model_folder", "."), stem)
-
-    if args_test.dataset in downstream.GRAPH_DSETS:
-        if len(gpus) > 1 or nodes_file:
-            raise SystemExit("whole-graph datasets are embedded on one GPU, every graph: --gpu takes one id and "
-                             "--nodes does not apply")
-        torch.cuda.set_device(gpus[0])
-        opt.device = torch.device("cuda", gpus[0])
-        encoder = GraphEncoder(degree_input=True, **{kw: getattr(opt, attr) for kw, attr in ENCODER_KWARGS.items()})
-        encoder.load_state_dict(ckpt["model"])
-        encoder = encoder.to(opt.device)
-        del ckpt
-        graphs = GraphClassificationDatasetLabeled(
-            downstream.graph_dataset_graphs(args_test.dataset), rw_hops=opt.rw_hops,
-            subgraph_size=opt.subgraph_size, restart_prob=opt.restart_prob,
-            positional_embedding_size=opt.positional_embedding_size, device=opt.device,
-            batch_size=args_test.batch_size)
-        emb = test_graphs(graphs, encoder, opt)
-        np.save(out, emb.numpy())
-        print("saved {} embeddings of dim {} to {}.npy".format(emb.shape[0], emb.shape[1], out))
-        return emb
-
+    whole = whole_graph_source(args_test.dataset) is not None
+    if getattr(args_test, "whole_graphs", False):
+        if not (args_test.dataset.endswith(".bin") or args_test.dataset.endswith(".npz")):
+            raise SystemExit("--whole-graphs embeds the graphs of a .bin or .npz corpus; %r is not one"
+                             % args_test.dataset)
+        whole = True
+    out = os.path.join(getattr(opt, "model_folder", "."), output_stem(args_test.dataset, whole))
     del ckpt
-    graph = resolve_graph(args_test.dataset, args_test.graph_nodes, args_test.graph_edges)
-    n_nodes = load_graphs(graph)[0].num_nodes
+
+    if whole:
+        graphs = resolve_whole_graphs(args_test.dataset)
+        n_items = len(graphs[1]) if isinstance(graphs, tuple) else len(graphs)
+        what = "graph"
+    else:
+        graph = resolve_graph(args_test.dataset, args_test.graph_nodes, args_test.graph_edges)
+        n_items = load_graphs(graph)[0].num_nodes
+        what = "node"
     ids = None
     if nodes_file:
         ids = read_nodes(nodes_file)
-        if ids.min() < 0 or ids.max() >= n_nodes:
-            raise SystemExit("%s: node ids must lie in 0..%d" % (nodes_file, n_nodes - 1))
-    n = n_nodes if ids is None else len(ids)
+        if ids.min() < 0 or ids.max() >= n_items:
+            raise SystemExit("%s: %s ids must lie in 0..%d" % (nodes_file, what, n_items - 1))
+    n = n_items if ids is None else len(ids)
     rows_of = (lambda lo, hi: range(lo, hi)) if ids is None else (lambda lo, hi: ids[lo:hi])
     out_file = out + ".npy"
     emb = np.lib.format.open_memmap(out_file, mode="w+", dtype=np.float32, shape=(n, opt.hidden_size))
-    B = min(args_test.batch_size, n_nodes)
+    B = min(args_test.batch_size, n_items)
     try:
         if len(gpus) == 1:
-            stats = [_node_rows(path, graph, args_test.batch_size, prefetch, gpus[0], rows_of(0, n), emb)]
+            stats = [_node_rows(path, graphs if whole else graph, args_test.batch_size, prefetch, gpus[0],
+                                rows_of(0, n), emb, whole)]
         else:
-            # shards aligned to the batches a one-GPU run makes, so every batch holds the same nodes
-            stats = _run_shards(args_test, gpus, split_shards(n, B, len(gpus)), rows_of, out_file, prefetch)
+            # shards aligned to the batches a one-GPU run makes, so every batch holds the same items
+            stats = _run_shards(args_test, gpus, split_shards(n, B, len(gpus)), rows_of, out_file, prefetch, whole)
         emb.flush()
     except BaseException:
         del emb
         os.remove(out_file)
         raise
     print("saved {} embeddings of dim {} to {}".format(n, opt.hidden_size, out_file))
-    print(replan_line(stats, -(-n // B)))
+    if whole:
+        print("whole graphs: batch buffers sized from the largest batch, up to %d vertices and %d edge entries"
+              % max(big for _, big in stats))
+    else:
+        print(replan_line(stats, -(-n // B)))
     return torch.from_numpy(np.asarray(emb))
 
 
@@ -287,8 +321,8 @@ def parse_args(argv=None):
     ap = argparse.ArgumentParser("inference export: node embeddings from a pretraining checkpoint")
     ap.add_argument("--load-path", type=str, required=True, help="path to load model")
     ap.add_argument("--dataset", type=str, default="synthetic-er",
-                    help="a downstream dataset (%s; files under ./data), an .npz CSR file (indptr, indices), a DGL "
-                         ".bin corpus or synthetic-er / synthetic-chunglu"
+                    help="a downstream dataset (%s; files under ./data), a TU directory, an .npz CSR file (indptr, "
+                         "indices), a DGL .bin corpus or synthetic-er / synthetic-chunglu"
                          % ", ".join(downstream.NODE_DSETS + downstream.GRAPH_DSETS))
     ap.add_argument("--graph-nodes", type=int, default=2000, help="size of a synthetic target graph")
     ap.add_argument("--graph-edges", type=int, default=10000)
@@ -298,7 +332,11 @@ def parse_args(argv=None):
     ap.add_argument("--prefetch", type=int, default=4,
                     help="batches whose sampling and positional features run ahead of the encoder; 0 = serial")
     ap.add_argument("--nodes", type=str, default=None,
-                    help="a .npy or text file of node ids: write only their rows, in the file's order")
+                    help="a .npy or text file of node ids (graph ids for whole graphs): write only their rows, in "
+                         "the file's order")
+    ap.add_argument("--whole-graphs", action="store_true",
+                    help="a .bin or .npz corpus: one row per graph (the whole graph, seed on its first maximum-degree "
+                         "vertex), saved as <stem>.graphs.npy")
     return ap.parse_args(argv)
 
 

@@ -44,6 +44,8 @@ typedef enum {
 #define GCCB_FLAG_EIG_NOCONV 8      /* eigensolver hit its sweep/iteration limit        */
 #define GCCB_FLAG_EIG_TOOBIG 16     /* ego-net larger than the eigensolver supports     */
 #define GCCB_FLAG_NONFINITE 32      /* gccb_knn: an input row holds a NaN or an Inf     */
+#define GCCB_FLAG_BAD_ROW 64        /* gccb_seed_first_union: a row is not non-decreasing
+                                       or names a vertex outside its graph              */
 
 int gccb_version(void);
 /* compute capability (major*10+minor) of the current device, or a negative status */
@@ -173,6 +175,18 @@ typedef struct {
  * gccb_sample_batch.  No workspace, no host sync.                                                       */
 int gccb_gather_graphs(const gccb_graph_set_t* set, const int64_t* graph_ids, const gccb_batch_t* batch,
                        gccb_stream_t stream);
+
+/* The graph set relabelled seed first, from `set` as given (indptr, indices, node_off read; edge_off is not: the
+ * output keeps the input's edge offsets).  n_nodes = node_off[n_graphs] <= 2^31 and n_edges = indptr[n_nodes] are
+ * the caller's host copies.  Per graph of n vertices: the seed s is its first vertex of maximum row length (parallel
+ * edges and self loops count); the new row order is [s, 0..s-1, s+1..n-1]; old local id u becomes 0 if u == s, u + 1
+ * if u < s and u otherwise.  Writes seeds[n_graphs] (local ids; 0 for a graph without vertices), out_indptr
+ * [n_nodes+1] and out_indices[n_edges], in union ids.  Rows must be non-decreasing (gccb_graph_t) and name vertices
+ * of their own graph; the relabelled rows are then non-decreasing too, byte for byte what relabelling each graph and
+ * sorting its rows gives.  A row that breaks this raises GCCB_FLAG_BAD_ROW in *flags (caller clears), and the
+ * output is undefined but written inside its rows.  One read and one write of the CSR; no workspace, no host sync. */
+int gccb_seed_first_union(const gccb_graph_set_t* set, int64_t n_nodes, int64_t n_edges, int64_t* seeds,
+                          int64_t* out_indptr, int32_t* out_indices, int32_t* flags, gccb_stream_t stream);
 
 /* A5  Laplacian positional features.  Replaces
  * _add_undirected_graph_positional_embedding + eigen_decomposision
