@@ -13,6 +13,11 @@ FLAG_NAMES = {1: "node capacity overflow", 2: "edge capacity overflow",
               16: "ego-net too large for the eigensolver"}
 FLAG_NONFINITE = 32                 # gccb_knn: an input row holds a NaN or an Inf
 FLAG_BAD_ROW = 64                   # gccb_seed_first_union: a row is not non-decreasing or leaves its graph
+FLAG_PROBE_NOCONV = 128             # gccb_probe_fit: a problem did not converge
+GCCB_PROBE_ACTIVE, GCCB_PROBE_CONVERGED, GCCB_PROBE_CONST_POS, GCCB_PROBE_CONST_NEG = 0, 1, 2, 3
+GCCB_PROBE_NOCONV, GCCB_PROBE_LS_FAIL, GCCB_PROBE_NOT_PD = 4, 5, 6
+PROBE_STATUS = {0: "active", 1: "converged", 2: "constant +inf", 3: "constant -inf", 4: "iteration limit",
+                5: "no step length met the Armijo condition", 6: "non-positive Cholesky pivot"}
 
 p = C.c_void_p
 
@@ -161,6 +166,11 @@ _PROTOS = {
     "gccb_knn_workspace": (C.c_size_t, [C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32]),
     "gccb_knn": (C.c_int, [p, C.c_int64, p, C.c_int64, C.c_int32, C.c_int32, p, C.c_int32, p, p, p, p, C.c_size_t,
                            p]),
+    "gccb_probe_workspace": (C.c_size_t, [C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
+    "gccb_probe_fit": (C.c_int, [p, C.c_int64, C.c_int32, p, C.c_int32, p, C.c_int32, C.c_double, C.c_int32,
+                                 C.c_int32, p, p, p, p, p, p, p, p, C.c_size_t, p]),
+    "gccb_probe_system": (C.c_int, [p, C.c_int64, C.c_int32, p, C.c_int32, p, C.c_int32, C.c_double, C.c_int32, p,
+                                    p, p, p, p, p, p, C.c_size_t, p]),
 }
 
 SYMBOLS = tuple(_PROTOS)

@@ -1,13 +1,15 @@
 """Frozen-embedding evaluators of the reference (gcc/tasks): node classification, graph classification and
 similarity search on the `.npy` rows generate.py writes.  They are scikit-learn fits on the host, as in the
-reference; at the datasets' sizes (a few thousand rows of 64) there is nothing for the GPU to do.  Similarity
-search over the millions of rows generate.py writes for a large graph is `gcc_b200.tasks.knn`, an exact cosine top-k
-on the GPU.
+reference, and stay there: at the named datasets' sizes (a few thousand rows of 64) a host fit takes seconds.  For
+the millions of rows generate.py writes for a large graph or corpus, the GPU has tools with an exact definition:
+`gcc_b200.tasks.knn`, a cosine top-k for similarity search, and `gcc_b200.tasks.linear_probe`, the node evaluator's
+one-vs-rest logistic regression (C = 1000) solved to a stated tolerance in float64, for node and graph labels.
 
     python -m gcc_b200.tasks.node_classification  --dataset usa_airport --model from_numpy --hidden-size 64 --emb-path <npy>
     python -m gcc_b200.tasks.graph_classification --dataset imdb-binary --model from_numpy_graph --hidden-size 64 --emb-path <npy>
     python -m gcc_b200.tasks.similarity_search    --dataset kdd_icdm --model from_numpy_align --hidden-size 64 \\
         --emb-path-1 <kdd.npy> --emb-path-2 <icdm.npy>
+    python -m gcc_b200.tasks.linear_probe         --dataset <name | y.npz | graph labels> --emb-path <npy>
 """
 import numpy as np
 

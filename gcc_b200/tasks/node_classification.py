@@ -1,6 +1,11 @@
 """Node classification on frozen embeddings (gcc/tasks/node_classification.py): one-vs-rest logistic regression
 (C = 1000) that predicts each test node's top-k labels, k = its label count, under a shuffled stratified 10-fold
-split of the argmax labels; the mean micro-F1 over the folds is reported as {"Micro-F1": ...}."""
+split of the argmax labels; the mean micro-F1 over the folds is reported as {"Micro-F1": ...}.
+
+`--dataset` is one of the five named node datasets (labels from data/, rows of the vertices that have edges, zeros
+elsewhere) or an .npz holding `y`, the finetune format (one label per row, or a 2-D 0/1 label matrix): its rows are
+the embedding file's rows as they are.  The same fit on the GPU, solved to a stated tolerance and at any size, is
+`gcc_b200.tasks.linear_probe`."""
 import argparse
 import warnings
 from collections import defaultdict
@@ -14,14 +19,22 @@ from sklearn.multiclass import OneVsRestClassifier
 
 from ..datasets.downstream import create_node_classification_dataset
 from . import build_model, edge_nodes
+from .linear_probe import label_matrix
 
 warnings.filterwarnings("ignore")
 
 
 class NodeClassification:
     def __init__(self, dataset, model, hidden_size, num_shuffle, seed, root="data", **model_args):
-        self.data = create_node_classification_dataset(dataset, root).data
-        self.label_matrix = self.data.y.numpy()
+        if dataset.endswith(".npz"):
+            self.data = None
+            with np.load(dataset) as z:
+                if "y" not in z.files:
+                    raise ValueError("%s holds no y" % dataset)
+                self.label_matrix = label_matrix(z["y"])
+        else:
+            self.data = create_node_classification_dataset(dataset, root).data
+            self.label_matrix = self.data.y.numpy()
         self.num_nodes, self.num_classes = self.label_matrix.shape
         self.model = build_model(model, hidden_size, **model_args)
         self.hidden_size = hidden_size
@@ -29,6 +42,14 @@ class NodeClassification:
         self.seed = seed
 
     def train(self):
+        if self.data is None:                                       # an .npz: the file's rows as they are
+            emb = getattr(self.model, "emb", None)
+            if emb is not None and len(emb) != self.num_nodes:
+                raise ValueError("%d embedding rows for %d label rows: the rows must be one per node, in order"
+                                 % (len(emb), self.num_nodes))
+            nodes = np.arange(self.num_nodes)
+            return self._evaluate(np.asarray(self.model.train(nodes), np.float64), self.label_matrix,
+                                  self.num_shuffle)
         nodes = edge_nodes(self.data.edge_index.numpy())
         features_matrix = np.zeros((self.num_nodes, self.hidden_size))
         features_matrix[nodes] = self.model.train(nodes)

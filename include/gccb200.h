@@ -46,6 +46,8 @@ typedef enum {
 #define GCCB_FLAG_NONFINITE 32      /* gccb_knn: an input row holds a NaN or an Inf     */
 #define GCCB_FLAG_BAD_ROW 64        /* gccb_seed_first_union: a row is not non-decreasing
                                        or names a vertex outside its graph              */
+#define GCCB_FLAG_PROBE_NOCONV 128  /* gccb_probe_fit: a problem did not converge
+                                       (iteration limit, line search or a non-positive pivot) */
 
 int gccb_version(void);
 /* compute capability (major*10+minor) of the current device, or a negative status */
@@ -577,6 +579,57 @@ size_t gccb_knn_workspace(int64_t nq, int64_t nc, int32_t dim, int32_t k, int32_
 int gccb_knn(const float* queries, int64_t nq, const float* cands, int64_t nc, int32_t dim, int32_t k,
              const int64_t* exclude, int32_t splits, int64_t* out_ids, float* out_scores, int32_t* flags, void* ws,
              size_t ws_bytes, gccb_stream_t stream);
+
+/* ---- linear-probe classification: exact one-vs-rest logistic regression (csrc/probe.cu) ------------------------
+ * The reference's node evaluator (gcc/tasks/node_classification.py) fits OneVsRestClassifier(LogisticRegression(
+ * C=1000)) on the host; this is the same model, solved to a stated tolerance, at the sizes generate.py writes.
+ *   x [n][d]: fp32 rows, 1 <= d <= 256, each value used exactly in float64.  y [n][c]: 0/1 bytes, 1 <= c <= 1024.
+ *   fold [n]: the test fold of each row, 0 .. folds-1 (1 <= folds <= 64); a row with any other id is in no test set
+ *   and trains every problem.
+ *   Problem p = f c + j (fold f, class j), on the training rows of f (fold id != f), targets t_i = y[i][j]:
+ *     minimise 1/2 |w|^2 + C sum_i log(1 + exp(-s_i (w.x_i + b))), s_i = 2 t_i - 1, b not penalised.
+ *   If every training row has the same target the problem is a constant predictor: decision value +inf or -inf,
+ *   status GCCB_PROBE_CONST_POS / _NEG, w = 0.  Otherwise damped Newton in float64 from w = 0, b = 0: the exact
+ *   gradient and Hessian [X 1]^T diag(C p (1-p)) [X 1] + diag(I_d, 0), a Cholesky solve, and the first step length
+ *   alpha = 2^-m, m = 0..15, with f(w + alpha dw) <= f(w) + 1e-4 alpha g.dw + 1e-12 |f(w)| (the last term absorbs
+ *   the rounding of f itself); a pass evaluates four consecutive lengths, and a problem that needs more continues
+ *   along the same step in the next pass.  Stop when |g|_inf <= 1e-10 max(1, |g at w = 0|_inf).  A problem still
+ *   active after max_iter passes, that finds no step length or that meets a non-positive pivot ORs
+ *   GCCB_FLAG_PROBE_NOCONV into *flags.
+ *   z(i, j) = the sequential fma chain of w_k x_ik over k = 0 .. d-1 from +0, plus b, with the weights of problem
+ *   (fold[i], j): decision values z [n][c] (float64).  Each test row with k labels predicts the k classes of largest
+ *   z, ties to the lower class; counts [folds][3] = (tp, fp, fn) per fold.
+ *   w [folds c][d + 1]: the weights, b last.  status, gnorm (the final |g|_inf), iters: [folds c].
+ * Every sum has a fixed order that depends only on n, d and the problem (row splits chosen from n and merged in
+ * order), so the outputs are a function of the inputs: they do not depend on `batch`, the problems per launch
+ * (0: all), or on the device.  A row holding a NaN or an Inf ORs GCCB_FLAG_NONFINITE into *flags and the call
+ * returns before fitting.  The call reads the count of active problems back to the host once per pass, so it
+ * synchronises `stream` and is not graph-capturable.
+ * Workspace, in bytes, 16-byte aligned, with P = folds c, B = the problems per launch, d1 = d + 1, D = d1 rounded
+ * up to 8, T = (D/8)(D/8 + 1)/2, S = min(64, ceil(n / 65536)), A(b) = b rounded up to 256:
+ *   3 A(4P) + A(8) + A(8P) + A(8 folds) + A(8c) + 3 A(8P) + A(8 P d1) + A(8 S B d1) + A(8 S B) + A(32 S B)
+ *   + A(512 S B T) + (d > 128 ? A(8 B d1^2) : 0).
+ * gccb_probe_workspace returns 0 for shapes gccb_probe_fit refuses.
+ * gccb_probe_system: for every problem at the given weights w, the gradient g_out [P][d1], the Hessian h_out
+ * [P][d1][d1], the Newton step step_out [P][d1] and the objective f_out [P], as one Newton iteration forms them
+ * (status [P] is written: GCCB_PROBE_NOT_PD where the Cholesky meets a non-positive pivot; the step is then
+ * undefined; no flag is raised).                                                                                  */
+#define GCCB_PROBE_ACTIVE 0
+#define GCCB_PROBE_CONVERGED 1
+#define GCCB_PROBE_CONST_POS 2
+#define GCCB_PROBE_CONST_NEG 3
+#define GCCB_PROBE_NOCONV 4
+#define GCCB_PROBE_LS_FAIL 5
+#define GCCB_PROBE_NOT_PD 6
+size_t gccb_probe_workspace(int64_t n, int32_t d, int32_t c, int32_t folds, int32_t batch);
+int gccb_probe_fit(const float* x, int64_t n, int32_t d, const uint8_t* y, int32_t c, const int32_t* fold,
+                   int32_t folds, double C, int32_t max_iter, int32_t batch, double* w, double* z, int64_t* counts,
+                   int32_t* status, double* gnorm, int32_t* iters, int32_t* flags, void* ws, size_t ws_bytes,
+                   gccb_stream_t stream);
+int gccb_probe_system(const float* x, int64_t n, int32_t d, const uint8_t* y, int32_t c, const int32_t* fold,
+                      int32_t folds, double C, int32_t batch, const double* w, double* g_out, double* h_out,
+                      double* step_out, double* f_out, int32_t* status, void* ws, size_t ws_bytes,
+                      gccb_stream_t stream);
 
 #ifdef __cplusplus
 }
