@@ -1,6 +1,6 @@
 """GPU (H100): the SGD and Adagrad optimisers (--optimizer sgd|adagrad, train.py:659-678) through the module
 API, PretrainEngine and train.py, against the golden fixtures of the real reference, the CPU oracle step, the
-float64 update formula and real torch.optim optimisers."""
+float64 update formula and real torch.optim optimisers; and the default Adam step against its float64 formula."""
 import os
 
 import numpy as np
@@ -218,6 +218,66 @@ def test_engine_update_matches_float64_formula(kind, moco, H, L):
             assert np.allclose(got_e, 0.999 * e0 + 0.001 * p1, rtol=1e-5, atol=1e-7), step
         else:
             assert np.array_equal(got_e, e0)                 # E2E: no momentum encoder
+    assert eng.adam_t == 4
+
+
+@pytest.mark.parametrize("moco,H,L", [(True, 64, 5), (True, 256, 3)], ids=["fp32", "wgmma"])
+def test_engine_adam_update_matches_float64_formula(moco, H, L):
+    """The default optimiser: the Adam update the engine applies against the float64 formula computed from its own
+    gradient buffer and its pre-step weights, adam_m, adam_v and EMA, with the step's lr and bias corrections read
+    from `hyper` (which must hold lr, 1 - beta1^t and sqrt(1 - beta2^t) in fp32).  Each entry is held to a bound
+    from the fp32 arithmetic of AdamRule: 16 U on the clipped, decayed gradient (the clip coefficient comes from a
+    rounded norm), 8 U on each moment's terms, their propagation through m / (sqrt(v) / sbc2 + eps), 8 U on the step
+    and on the weight."""
+    U = 2.0 ** -24
+    eng, model, ema, contrast = _engine("adam", moco, H, L, prefetch=4, opt_kw={})
+    assert bool(model.cfg.tensor_cores) == (H >= 128)
+    n_live, n_all = model.n_live, model._n_all
+    lr = 0.005
+    # the betas, eps and the EMA alpha as the kernel receives them (fp32); 1 - beta is exact in fp32 (Sterbenz)
+    b1, b2, eps, alpha = (float(np.float32(x)) for x in (0.9, 0.999, 1e-8, 0.999))
+    for step in range(4):
+        torch.cuda.synchronize()
+        p0 = model.flat_params[:n_all].double()
+        e0 = ema.flat_params[:n_all].double()
+        m0, v0 = eng.adam_m.double(), eng.adam_v.double()
+        eng.step(lr=lr)
+        s = eng.read_stats()
+        torch.cuda.synchronize()
+        t = step + 1
+        hyper = eng.hyper.double().cpu().numpy()
+        assert hyper[0] == np.float32(lr) and hyper[1] == np.float32(1 - 0.9 ** t)
+        assert hyper[2] == np.float32(np.sqrt(1 - 0.999 ** t))
+        lr_h, bc1, sbc2 = (float(x) for x in hyper[:3])
+        g = eng.grads.double()
+        total = float(torch.sqrt((g * g).sum()))
+        assert np.isclose(s["grad_norm"], total, rtol=1e-5)
+        coef = min(1.0, 1.0 / (total + 1e-6))
+        pl = p0[:n_live]
+        d = coef * g + 1e-5 * pl
+        ad = coef * g.abs() + 1e-5 * pl.abs()
+        err_d = 16 * U * ad
+        m1 = b1 * m0 + (1 - b1) * d
+        v1 = b2 * v0 + (1 - b2) * d * d
+        err_m = (1 - b1) * err_d + 8 * U * (b1 * m0.abs() + (1 - b1) * ad)
+        err_v = (1 - b2) * 2 * ad * err_d + 8 * U * (b2 * v0 + (1 - b2) * ad * ad)
+        den = v1.sqrt() / sbc2 + eps
+        stp = lr_h / bc1 * m1 / den
+        rel_sqrt = torch.where(v1 > 0, err_v / (2 * v1), torch.zeros_like(v1))
+        err_p = 8 * U * (pl.abs() + stp.abs()) + lr_h / bc1 * (err_m + m1.abs() * rel_sqrt) / den
+        p1 = torch.cat([pl - stp, p0[n_live:]])
+        got_m, got_v = eng.adam_m.double(), eng.adam_v.double()
+        got_p = model.flat_params[:n_all].double()
+        for name, got, want, bound in (("m", got_m, m1, err_m), ("v", got_v, v1, err_v),
+                                       ("p", got_p[:n_live], p1[:n_live], err_p)):
+            ratio = float(((got - want).abs() / (bound + 1e-30)).max())
+            print("adam %s step %d %s: worst |err| / bound = %.3g" % ("fp32" if H < 128 else "wgmma", step, name,
+                                                                      ratio))
+            assert ratio <= 1.0, (step, name, ratio)
+        assert torch.equal(got_p[n_live:], p0[n_live:])
+        got_e = ema.flat_params[:n_all].double()
+        want_e = alpha * e0 + (1 - alpha) * got_p
+        assert ((got_e - want_e).abs() <= 4 * U * (alpha * e0.abs() + (1 - alpha) * got_p.abs()) + 1e-30).all(), step
     assert eng.adam_t == 4
 
 
